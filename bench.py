@@ -1,9 +1,11 @@
 #!/usr/bin/env python
 """bench.py — HNSW k-NN queries/sec on synthetic f32 vectors (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--dump-outputs DIR]
 
 A step = one pass of the hot path (batched hnsw_knn) over one batch of B queries.
+--dump-outputs DIR writes what the last timed step returned as DIR/<name>.npy (float32 / float64); the inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 
 Workloads (SURVEY.md §8d):
   config2   (default) BASELINE configs[1]: 1M x 768 f32 per GPU, ef=200, k=10, batch 4096, index m=16 /
@@ -12,7 +14,8 @@ Workloads (SURVEY.md §8d):
             operator runs through the C ABI (cozo_gpu_hnsw_search_sharded[_dev]): per-shard search ->
             exchange (fused peer stores, or ONE NCCL all-gather per list with --exchange nccl) -> merge.
   config3   BASELINE configs[2]: 10M x 768, k=100, batch 65536, one GPU (roofline capture).
-  config5   BASELINE configs[4]: 12.5M x 768 per GPU (100M over 8), ef=200, k=10, batch 1M tiled by 65536.
+  config5   BASELINE configs[4]: 12.5M x 768 per GPU (100M over 8), ef=200, k=10, batch 1M tiled by 65536
+            (38 GB of vectors per GPU: fits an 80 GB H100 with the index and the query batches).
   strong10m SURVEY §8d strong-scaling series: 10M x 768 in total, split over the N GPUs, batch 65536.
   pagerank  BASELINE configs[3]: PageRank on RMAT scale 24 (separate metric, see run_pagerank).
 
@@ -79,10 +82,14 @@ def parse():
     ap.add_argument("--device-gen", type=int, default=-1, help="1/0: generate the corpus in HBM / on the host (-1: HBM above 2M rows)")
     ap.add_argument("--out", default=None, help="--impl export-graph: where to write the graph")
     ap.add_argument("--scale", type=int, default=24, help="pagerank: RMAT scale")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float32/float64, <= 64 MB)")
     ap.add_argument("--watchdog-s", type=int, default=int(os.environ.get("COZO_BENCH_WATCHDOG_S", 840)),
                     help="end the process (rc 3) if the run has not finished after this many seconds: a wedged kernel "
                          "must not hold the GPU box until the caller's limit (0 = off)")
     a = ap.parse_args()
+    if a.steps < 1 or a.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if a.workload in WORKLOADS:
         rows, batch, k, tile, scaling = WORKLOADS[a.workload]
         world = int(os.environ.get("WORLD_SIZE", 1))
@@ -128,10 +135,11 @@ def gen_vectors_dev(n, dim, seed, dev):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region, with the card's name and power limit
+    (a rate is only meaningful next to what it was measured on)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,name,power.limit")
 
     def __init__(self, gpu_index):
         self.rows = []
@@ -156,13 +164,18 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
-        sm, smax, reasons = [], None, set()
+        sm, smax, reasons, gpu, plim = [], None, set(), None, None
         for t, line in self.rows:
             if t < t0 - 0.05 or t > t1 + 0.15:
                 continue
             f = [x.strip() for x in line.split(",")]
-            if len(f) < 8:
+            if len(f) < 10:
                 continue
+            gpu = f[8]
+            try:
+                plim = float(f[9])
+            except ValueError:
+                pass
             try:
                 sm.append(float(f[1]))
                 smax = float(f[2])
@@ -172,7 +185,7 @@ class ClockSampler:
                 if v.lower().startswith("active"):
                     reasons.add(name)
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": smax, "reasons": sorted(reasons),
-                "samples": len(sm)}
+                "samples": len(sm), "gpu": gpu, "power_limit_w": plim}
 
 
 def peak_hbm():
@@ -180,17 +193,29 @@ def peak_hbm():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s; not measured)"
 
 
-def ncu_traffic(key="hnsw_search_bytes_per_launch"):
-    """dram bytes per launch of the dominant kernel from the committed ncu capture (not measurable inside
-    an un-profiled run); None when the capture does not cover this workload."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        return json.load(open(p)).get(key)
-    except Exception:
-        return None
+DUMP_BYTES = 60 << 20
+
+
+def dump_rows(n_rows, row_bytes):
+    """rows written by --dump-outputs: all of them, or a fixed seeded sample (ascending) that keeps the dump
+    under DUMP_BYTES"""
+    cap = DUMP_BYTES // row_bytes
+    if n_rows <= cap:
+        return np.arange(n_rows)
+    return np.sort(np.random.default_rng(0x5EED0005).choice(n_rows, cap, replace=False))
+
+
+def dump_outputs(d, arrays):
+    """--dump-outputs: one DIR/<name>.npy per array, float32 or float64 (ids as float64: exact for every id)"""
+    os.makedirs(d, exist_ok=True)
+    for name, v in arrays.items():
+        v = np.asarray(v)
+        if v.dtype != np.float32:
+            v = v.astype(np.float64)
+        np.save(os.path.join(d, name + ".npy"), v)
 
 
 def host_cores() -> int:
@@ -406,12 +431,15 @@ def run_pagerank(a):
                    "gen_s": round(gen_s, 2), "stage_s": round(stage_s, 2),
                    "options": {o.split("=")[0]: int(o.split("=")[1]) for o in a.opt}},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": ncu_traffic("pagerank_bytes_per_iteration"), "kernel": "pagerank iteration (all launches)",
+                     "kernel": "pagerank iteration (all launches)",
                      "algorithmic_bytes_per_iteration": bytes_iter, "peak_source": peak_src},
         "cpu_baseline": cpu,
         "e2e": {"value": m * iters / min(e2e_t), "unit": "edges/s", "h2d_bytes_per_step": 8 * m,
                 "d2h_bytes_per_step": 4 * n, "seconds_per_call": min(e2e_t)},
         "clocks": clocks, "gpu_launches": int(capi.get_option("pagerank.last_launches")) * a.steps}), flush=True)
+    if a.dump_outputs:        # the scores of the last timed call (sampled nodes above 5M)
+        sel = dump_rows(n, 4 + 8)
+        dump_outputs(a.dump_outputs, {"pagerank_scores": scores[sel], "pagerank_nodes": sel})
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -448,7 +476,7 @@ def main():
     import torch
     from cozo_b200 import capi
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: there is no CPU fallback for the hot path")
+        raise SystemExit("bench.py needs an H100: there is no CPU fallback for the hot path")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -534,6 +562,12 @@ def main():
     if world > 1:
         dist.barrier()
     clocks = sampler.stop(t_start, t_end)
+    if rank == 0 and a.dump_outputs:    # the last timed step's lists, before anything else reuses these buffers
+        sel = dump_rows(B, k * (8 + 4) + 8)
+        rows = torch.from_numpy(sel).to(dev)
+        dump_outputs(a.dump_outputs, {"knn_ids": (ids if grp is None else out_i)[rows].cpu().numpy(),
+                                      "knn_dist": (dd if grp is None else out_d)[rows].cpu().numpy(),
+                                      "knn_query_rows": sel})
     total_ms = e_all0.elapsed_time(e_all1)
     if world > 1:
         t = torch.tensor([total_ms], dtype=torch.float64, device=dev)
@@ -592,9 +626,6 @@ def main():
     achieved = alg_bytes_per_step / (kern_ms / 1e3) / 1e9
     tiles = -(-B // a.tile)
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": ncu_traffic() if a.workload == "config2" else None,
-                "traffic_source": "profiles/traffic.json (ncu --set full capture of this kernel at this workload; "
-                                  "not re-measured in this run)" if a.workload == "config2" else None,
                 "kernel": "hnsw_search_kernel", "kernel_ms": kern_ms,
                 "algorithmic_bytes_per_launch": alg_bytes_per_step / (tiles if world > 1 else 1),
                 "launches_per_step": tiles if world > 1 else 1, "peak_source": peak_src,
@@ -707,7 +738,7 @@ def main():
             "ms_per_step": total_ms / a.steps, "higher_is_better": True, "scaling": a.scaling, "vs_baseline": None,
             "dtype": "f32", "data": "synthetic",
             "config": {"workload": workload_name(a, world), "name": a.workload, "l2_policy": "inputs larger than L2 (corpus "
-                       f"{a.n * a.dim * 4 / 1e9:.2f} GB/GPU >> 126 MB), {nsets} distinct query batch(es) cycled per step",
+                       f"{a.n * a.dim * 4 / 1e9:.2f} GB/GPU >> 50 MB), {nsets} distinct query batch(es) cycled per step",
                        "value_counts": ("per-shard k-NN searches per second summed over ranks (== queries/s at N=1); "
                                         "global queries/s over the whole sharded corpus = value / n_gpus")
                        if a.scaling == "weak" else "global queries/s over the fixed corpus",

@@ -1,7 +1,8 @@
-"""In-tree build of libcozo_gpu.so (sm_100a only) with nvcc.
+"""In-tree build of libcozo_gpu.so (sm_90a, H100, only) with nvcc.
 
 `python -m cozo_b200.build` or cozo_b200.build.build().  The library is placed at
-cozo_b200/csrc/libcozo_gpu.so so that it travels to the GPU box with the snapshot.
+cozo_b200/csrc/libcozo_gpu.so, next to the sources, so that the package runs from the repository tree.
+Objects are rebuilt when a source, a header or this file (the flags) is newer than they are.
 """
 from __future__ import annotations
 
@@ -16,8 +17,9 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(CSRC, "libcozo_gpu.so")
 SOURCES = ["common.cu", "hnsw.cu", "hnsw_f64.cu", "hnsw_build.cu", "graph.cu", "pagerank.cu", "merge.cu", "sharded.cu"]
 HEADERS = ["common.cuh", "hnsw_device.cuh", "hnsw_host.hpp", "graph_host.hpp", "pagerank_pb.cuh", "graph_kernels.cuh", "hnsw_build_kernels.cuh", os.path.join("..", "..", "include", "cozo_gpu.h")]
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [
+    "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
 ]
 
@@ -46,7 +48,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     for s in srcs:
         src = os.path.join(CSRC, s)
         obj = os.path.join(objdir, s.replace(".cu", ".o"))
-        if force or _stale(obj, [src] + hdrs):
+        if force or _stale(obj, [src] + hdrs + [os.path.abspath(__file__)]):
             jobs.append((src, obj))
 
     def compile_one(job):
@@ -64,7 +66,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
                     print(log, file=sys.stderr)
     objs = [os.path.join(objdir, s.replace(".cu", ".o")) for s in srcs]
     if force or jobs or _stale(OUT, objs):
-        cmd = [nvcc, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static", "-ldl"]
+        cmd = [nvcc, "-shared", "-o", OUT] + objs + ARCH + ["-cudart", "static", "-ldl"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -3,7 +3,7 @@
 This is the Python twin of the Rust `extern "C"` block shown in INTEGRATION.md;
 tests, bench.py and smoke() drive the product exclusively through it.  The
 library is loaded from cozo_b200/csrc (in-tree) and there is no fallback: if it
-is missing or no sm_100 device is usable, calls raise CozoGpuError.
+is missing or no sm_90 device is usable, calls raise CozoGpuError.
 """
 from __future__ import annotations
 

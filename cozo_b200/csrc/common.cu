@@ -42,8 +42,8 @@ static int do_init(int device) {
   if (device < 0 || device >= count) return set_error(COZO_GPU_EINVAL, "device %d out of range [0,%d)", device, count);
   cudaDeviceProp prop;
   COZO_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return set_error(COZO_GPU_ENODEV, "device %d is sm_%d%d; this library is built for sm_100a only", device,
+  if (prop.major != 9 || prop.minor != 0)
+    return set_error(COZO_GPU_ENODEV, "device %d is sm_%d%d; this library is built for sm_90a only", device,
                      prop.major, prop.minor);
   COZO_CUDA(cudaSetDevice(device));
   COZO_CUDA(cudaFree(0));

@@ -1,5 +1,5 @@
 // common.cuh — error plumbing, options and small device helpers shared by the
-// kernels of libcozo_gpu.so (sm_100a only).
+// kernels of libcozo_gpu.so (sm_90a only).
 #pragma once
 // Two test-only build modes exist besides nvcc (tests/emu is test infrastructure; the product is always
 // built by nvcc): COZO_CPU_EMU = a harness compiles device headers only; COZO_CPU_EMU_LIB = the whole library is

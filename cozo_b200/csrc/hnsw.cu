@@ -283,10 +283,8 @@ static KernelFn pick_nv(uint32_t need, int metric, bool bulk) {
   return nullptr;
 }
 
-// 4 CTAs x 4 warps per SM (<= 128 registers).  Builds capped for more resident warps were measured
-// slower per 4096-query batch at 1M x 768 (profiles/r01_sweep3_minblocks.txt): 5 CTAs / 96 regs 12.3 ms,
-// 6 CTAs / 80 regs 14.9 ms, 7 CTAs / 72 regs 17.5 ms, vs 12.1-12.2 ms here: the batch is bandwidth-bound,
-// and the tighter register budgets cost instructions.
+// 4 CTAs x 4 warps per SM (<= 128 registers).  The batch is bandwidth-bound; builds capped for more resident
+// warps buy occupancy with tighter register budgets, which cost instructions (tools/sweep.py compares them).
 static KernelFn pick_kernel(uint32_t ld, int metric, bool bulk) {
   uint32_t need = (ld / 4 + 31) / 32;
   return pick_nv<4>(need, metric, bulk);
@@ -418,8 +416,8 @@ int hnsw_launch_search(cozo_gpu_hnsw* h, HnswWorkspace* ws, const float* d_q, ui
   uint32_t ns = (uint32_t)get_option("hnsw.stages", 4);
   if (ns < 1) ns = 1;
   if (ns > 32) ns = 32;
-  // measured crossover at 1M x 768 (profiles/r01_batch_sweep_1Mx768.txt): the cooperative kernel wins up to
-  // about 1.5 waves of CTAs (592 resident), the warp-per-query kernel beyond
+  // the cooperative kernel wins while the batch is below about 1.5 waves of its CTAs (4 resident per SM), the
+  // warp-per-query kernel beyond (tools/sweep_batch.py measures the crossover)
   const uint32_t coop_below = (uint32_t)get_option("hnsw.coop_below", (int64_t)di.sm_count * 6);
   if (mode < 0) mode = B < coop_below ? 2 : 1;
   SearchParams p{};

@@ -1,5 +1,5 @@
 /*
- * cozo_gpu.h — C ABI of libcozo_gpu.so, the B200 (sm_100a) implementation of
+ * cozo_gpu.h — C ABI of libcozo_gpu.so, the H100 (sm_90a) implementation of
  * CozoDB's HNSW k-NN search and FixedRule graph algorithms.
  *
  * This is the drop-in boundary: every entry point below is what the reference's
@@ -15,7 +15,7 @@
  *   - ids are dense u32 assigned by the host (Rust) side, which keeps the
  *     id <-> (Tuple key, field, sub-index) table (CompoundKey, hnsw.rs:55) or the
  *     id <-> DataValue table (fixed_rule/mod.rs:144-145).
- *   - there is NO CPU fallback: without a usable sm_100 device init fails.
+ *   - there is NO CPU fallback: without a usable sm_90 device init fails.
  *   - search calls are re-entrant per handle: each call takes its own stream and
  *     a workspace from a bounded pool.  Graph algorithm calls are thread-safe per
  *     handle too (the staged graph is read-only, every call owns its buffers) but
@@ -40,7 +40,7 @@ extern "C" {
 #define COZO_GPU_OK 0
 #define COZO_GPU_EINVAL (-1)   /* bad argument (dimension mismatch, k==0, ...) */
 #define COZO_GPU_ECUDA (-2)    /* CUDA runtime / driver error                  */
-#define COZO_GPU_ENODEV (-3)   /* no sm_100 device / extension unusable        */
+#define COZO_GPU_ENODEV (-3)   /* no sm_90 device / extension unusable         */
 #define COZO_GPU_ENOMEM (-4)   /* allocation failed                            */
 #define COZO_GPU_EKILLED (-5)  /* poison flag was set (runtime/db.rs:1933-1941) */
 #define COZO_GPU_EUNSUP (-6)   /* outside the supported envelope (e.g. maintenance of an F64 index) */
@@ -54,7 +54,7 @@ extern "C" {
 #define COZO_GPU_IP 2     /* 1 - a.b                            */
 
 /* ---- lifecycle ---------------------------------------------------------- */
-/* Binds the calling process to `device` (ordinal) and verifies it is sm_100. */
+/* Binds the calling process to `device` (ordinal) and verifies it is sm_90. */
 int cozo_gpu_init(int device);
 void cozo_gpu_shutdown(void);
 const char* cozo_gpu_last_error(void);

@@ -45,7 +45,7 @@ pub(crate) fn ensure_device() -> Result<()> {
     });
     match r {
         Ok(()) => Ok(()),
-        Err(e) => Err(miette!("gpu-b200: no usable sm_100 device ({}); this build has no CPU path for this rule", e)),
+        Err(e) => Err(miette!("gpu-b200: no usable sm_90 device ({}); this build has no CPU path for this rule", e)),
     }
 }
 

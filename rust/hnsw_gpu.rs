@@ -373,7 +373,7 @@ impl<'a> SessionTx<'a> {
 }
 
 /// Parent tuples gathered per device call.  One launch amortises best from a few hundred queries
-/// up (profiles/r01_batch_sweep_1Mx768.json); smaller parents simply produce one short batch.
+/// up; smaller parents simply produce one short batch.
 const GPU_BATCH: usize = 4096;
 
 impl HnswSearchRA {

@@ -9,8 +9,8 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
-    config.addinivalue_line("markers", "gpu_unverified: needs a B200 AND exercises code that has not run on one yet "
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a GPU machine)")
+    config.addinivalue_line("markers", "gpu_unverified: needs an H100 AND exercises code that has not run on one yet "
                                        "(opt in with COZO_RUN_UNVERIFIED=1; never selected by -m gpu)")
 
 

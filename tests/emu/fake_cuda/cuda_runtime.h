@@ -2,7 +2,7 @@
 // (host code included) into libcozo_gpu_emu.so with g++ (tests/emu/build_emu_lib.py; TEST INFRASTRUCTURE ONLY).
 // Device memory is host memory, streams are synchronous, events are wall-clock stamps, a kernel launch is
 // emu::launch_dyn (cuda_emu.hpp: one OS thread per CUDA thread, blocks one after the other).  The "device" reports
-// itself as sm_100 with a handful of SMs so that persistent grids stay small.  Nothing under cozo_b200/ includes this.
+// itself as sm_90 with a handful of SMs so that persistent grids stay small.  Nothing under cozo_b200/ includes this.
 #pragma once
 #include "../cuda_emu.hpp"
 
@@ -44,7 +44,7 @@ struct cudaDeviceProp {
 
 namespace emu {
 inline thread_local cudaError_t t_last_error = cudaSuccess;
-inline constexpr size_t kSmemOptin = 232448;  // 227 KB, the B200 opt-in limit: the host code sizes tiles against it
+inline constexpr size_t kSmemOptin = 232448;  // 227 KB, the H100 opt-in limit: the host code sizes tiles against it
 inline int sm_count() {
   const char* e = getenv("COZO_EMU_SM_COUNT");
   return e && *e ? atoi(e) : 4;
@@ -71,8 +71,8 @@ inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 inline cudaError_t cudaDeviceSynchronize() { return cudaSuccess; }
 inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
   memset(p, 0, sizeof(*p));
-  strcpy(p->name, "CPU SIMT emulator (reports sm_100)");
-  p->major = 10;
+  strcpy(p->name, "CPU SIMT emulator (reports sm_90)");
+  p->major = 9;
   p->minor = 0;
   p->multiProcessorCount = emu::sm_count();
   p->sharedMemPerBlockOptin = emu::kSmemOptin;

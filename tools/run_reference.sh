@@ -1,11 +1,10 @@
 #!/bin/bash
-# Pin the oracle against the REAL reference (VERDICT r01 item 3).  Needs cargo + crates.io access, which neither
-# the build image nor the GPU boxes have (probed: profiles/r02_gpu_box_probe.txt) — run it on any machine with a
+# Pin the oracle against the REAL reference.  Needs cargo + crates.io access — run it on any machine with a
 # Rust toolchain and commit the two JSON files it writes; tests/test_oracle_cpu.py::test_reference_goldens then
 # compares the oracle with them (it skips while they are absent).
 #   usage: tools/run_reference.sh /path/to/cozo            (the repository root that holds cozo-core/)
 set -euo pipefail
-REF="${1:-/root/reference}"
+REF="${1:?usage: tools/run_reference.sh /path/to/cozo}"
 HERE="$(cd "$(dirname "$0")/.." && pwd)"
 command -v cargo >/dev/null || { echo "cargo not found: this script needs a Rust toolchain" >&2; exit 2; }
 TMP="$(mktemp -d)"
