@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(CSRC, "libcozo_gpu.so")
 SOURCES = ["common.cu", "hnsw.cu", "hnsw_f64.cu", "hnsw_build.cu", "graph.cu", "pagerank.cu", "merge.cu", "sharded.cu"]
-HEADERS = ["common.cuh", "hnsw_device.cuh", "hnsw_host.hpp", "graph_host.hpp", "pagerank_pb.cuh", "graph_kernels.cuh", "hnsw_build_kernels.cuh", os.path.join("..", "..", "include", "cozo_gpu.h")]
+HEADERS = ["common.cuh", "hnsw_codes.cuh", "hnsw_device.cuh", "hnsw_host.hpp", "graph_host.hpp", "pagerank_pb.cuh", "graph_kernels.cuh", "hnsw_build_kernels.cuh", os.path.join("..", "..", "include", "cozo_gpu.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [
     "-O3", "-lineinfo", "-std=c++17",

@@ -26,6 +26,7 @@ struct SearchParams {
   uint32_t ns;
   uint32_t warp_smem;  // bytes of shared memory per warp
   uint32_t off_fi, off_pend, off_bars, off_ring;
+  uint32_t cns, off_cbars, off_cring;  // code ring of the pruned search (cns = 0: none)
   // fused exchange of the sharded corpus: besides (or instead of) out_ids/out_dist the top-k of
   // query qi is stored into every destination's [n_slots][B][k] gather buffer at slot `slot`;
   // destinations are peer GPUs' buffers mapped over NVLink (plain st.global on peer pointers).
@@ -113,14 +114,21 @@ __global__ void __launch_bounds__(128, MINB) hnsw_search_kernel(HnswDev g, Searc
   w.nlog = 0;
   w.head = 0;
   w.phase = 0;
+  w.cring = base + p.off_cring;
+  w.cbars = reinterpret_cast<uint64_t*>(base + p.off_cbars);
+  w.cns = p.cns;
+  w.chead = 0;
+  w.cphase = 0;
   if (BULK) {
     if (lane == 0) {
       for (uint32_t s = 0; s < p.ns; ++s) mbar_init(&w.bars[s], 1);
+      for (uint32_t s = 0; s < p.cns; ++s) mbar_init(&w.cbars[s], 1);
       mbar_fence_init();
     }
     __syncwarp();
   }
   const int nvec4 = g.ld >> 2;
+  constexpr bool PRUNE = BULK && METRIC == COZO_GPU_L2;  // at run time: only if g.codes is set (then p.cns > 0)
 
   for (;;) {
     uint32_t qi = 0;
@@ -132,7 +140,7 @@ __global__ void __launch_bounds__(128, MINB) hnsw_search_kernel(HnswDev g, Searc
     load_query<NV>(p.queries + (size_t)qi * g.dim, g.dim, lane, q, qnorm);
     w.len = 0;
     w.cursor = 0;
-    w.dist_evals = w.nodes_expanded = w.nbr_reads = 0;
+    w.dist_evals = w.nodes_expanded = w.nbr_reads = w.pruned = 0;
     uint32_t found = 0;
     if (g.entry != NONE) {  // empty index => no rows (hnsw.rs:903-909)
       // entry point distance (hnsw.rs:915-918)
@@ -146,14 +154,14 @@ __global__ void __launch_bounds__(128, MINB) hnsw_search_kernel(HnswDev g, Searc
       w.len = 1;
       __syncwarp();
       for (uint32_t lvl = g.top_level; lvl >= 1; --lvl)  // hnsw.rs:919-929
-        search_level<NV, METRIC, BULK>(g, w, q, qnorm, 1, lvl, lane);
-      search_level<NV, METRIC, BULK>(g, w, q, qnorm, p.ef, 0, lane);  // hnsw.rs:930-938
+        search_level<NV, METRIC, BULK, PRUNE>(g, w, q, qnorm, 1, lvl, lane);
+      search_level<NV, METRIC, BULK, PRUNE>(g, w, q, qnorm, p.ef, 0, lane);  // hnsw.rs:930-938
     }
     found = emit_results(p, w, qi, lane, g.entry != NONE);
     if (lane == 0) {
       if (p.out_count) p.out_count[qi] = found;
       if (p.qstats) {
-        uint4 s = make_uint4(w.dist_evals, w.nodes_expanded, w.nbr_reads, 0);
+        uint4 s = make_uint4(w.dist_evals, w.nodes_expanded, w.nbr_reads, w.dist_evals - w.pruned);
         reinterpret_cast<uint4*>(p.qstats)[qi] = s;
       }
     }
@@ -231,7 +239,8 @@ __global__ void __launch_bounds__(128, 4) hnsw_search_coop_kernel(HnswDev g, Sea
       found = emit_results(p, w, qi, lane, g.entry != NONE);
       if (lane == 0) {
         if (p.out_count) p.out_count[qi] = found;
-        if (p.qstats) reinterpret_cast<uint4*>(p.qstats)[qi] = make_uint4(w.dist_evals, w.nodes_expanded, w.nbr_reads, 0);
+        if (p.qstats)  // every evaluated row is fetched: the fourth word equals dist_evals
+          reinterpret_cast<uint4*>(p.qstats)[qi] = make_uint4(w.dist_evals, w.nodes_expanded, w.nbr_reads, w.dist_evals);
       }
     }
     __syncthreads();
@@ -404,6 +413,47 @@ static void free_ws(HnswWorkspace* ws) {
   delete ws;
 }
 
+static void codes_drop(cozo_gpu_hnsw* h) {
+  if (h->d_codes) cudaFree(h->d_codes);
+  h->d_codes = nullptr;
+  h->codes_rows = 0;
+  h->codes_failed = true;
+  h->dev.codes = nullptr;
+}
+
+// Room for `rows` code rows, keeping rows [0, n).  Only L2 f32 indexes with ld >= CODES_MIN_LD carry codes.  A failed
+// allocation leaves
+// the index without codes: it is then searched without pruning, with the same results.
+void hnsw_codes_reserve(cozo_gpu_hnsw* h, uint32_t rows) {
+  HnswDev& g = h->dev;
+  if (h->f64 || g.metric != COZO_GPU_L2 || g.ld < CODES_MIN_LD || h->codes_failed || rows <= h->codes_rows) return;
+  uint8_t* nc = nullptr;
+  if (cudaMalloc(&nc, (size_t)rows * g.code_ld) != cudaSuccess) {
+    cudaGetLastError();  // not sticky: clear it
+    codes_drop(h);
+    return;
+  }
+  if (h->d_codes && g.n && cudaMemcpy(nc, h->d_codes, (size_t)g.n * g.code_ld, cudaMemcpyDeviceToDevice) != cudaSuccess) {
+    cudaGetLastError();
+    cudaFree(nc);
+    codes_drop(h);
+    return;
+  }
+  if (h->d_codes) cudaFree(h->d_codes);
+  h->d_codes = nc;
+  h->codes_rows = rows;
+  g.codes = nc;
+}
+
+// Re-quantise the code rows of the vector rows just written (ids = nullptr: rows first .. first+count-1), on the
+// default stream, after the writes to d_vec.
+void hnsw_codes_fill(cozo_gpu_hnsw* h, uint32_t first, uint32_t count, const uint32_t* d_ids) {
+  const HnswDev& g = h->dev;
+  if (!g.codes || !count) return;
+  quantize_rows_kernel<<<(count + 127) / 128, 128>>>(h->d_vec, g.ld, h->d_codes, d_ids, first, count);
+  if (cudaGetLastError() != cudaSuccess) codes_drop(h);
+}
+
 int hnsw_launch_search(cozo_gpu_hnsw* h, HnswWorkspace* ws, const float* d_q, uint32_t B, uint32_t k, uint32_t ef,
                        double radius, uint32_t* d_ids, float* d_dist, uint32_t* d_count, uint32_t* d_qstats,
                        cudaStream_t stream, const ScatterDest* scatter, const uint32_t* d_filter_mask) {
@@ -459,6 +509,19 @@ int hnsw_launch_search(cozo_gpu_hnsw* h, HnswWorkspace* ws, const float* d_q, ui
     p.off_bars = p.off_pend + 32 * 4;
     p.off_ring = round_up(p.off_bars + ns * 8, 128);
     p.warp_smem = round_up(p.off_ring + ns * g.ld * 4, 128);
+    if (bulk && g.codes) {
+      // pruned search (code_prune): most rows of a hop never reach the f32 ring, so it keeps at most 2 stages and
+      // the code ring takes the rest of the same per-warp budget; the CTAs resident per SM stay what they were.
+      // [fd][fi][pend][bars ns][code bars <= 16][f32 ring ns][code ring cns]
+      const uint32_t budget = p.warp_smem;
+      ns = std::min<uint32_t>(ns, 2);
+      p.off_cbars = p.off_bars + ns * 8;
+      p.off_ring = round_up(p.off_cbars + 16 * 8, 128);
+      p.off_cring = p.off_ring + ns * g.ld * 4;  // a multiple of 16: ld is a multiple of 4
+      const uint32_t room = budget > p.off_cring ? budget - p.off_cring : 0;
+      p.cns = std::min<uint32_t>(16, std::max<uint32_t>(2, room / g.code_ld));
+      p.warp_smem = round_up(p.off_cring + p.cns * g.code_ld, 128);
+    }
     smem = (size_t)p.warp_smem * wpc;
     while (smem > di.smem_optin && wpc > 1) {
       wpc >>= 1;
@@ -643,6 +706,9 @@ extern "C" int cozo_gpu_hnsw_stage(cozo_gpu_hnsw_t** out, const CozoGpuHnswStage
                             d->vectors_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
   }
   g.vec = h->d_vec;
+  g.code_ld = code_row_bytes(g.ld);
+  hnsw_codes_reserve(h, n);
+  hnsw_codes_fill(h, 0, n);
   // layer 0 adjacency
   {
     std::vector<uint32_t> adj((size_t)n * g.s0, NONE);
@@ -694,6 +760,7 @@ extern "C" void cozo_gpu_hnsw_free(cozo_gpu_hnsw_t* h) {
   if (!h) return;
   for (auto* ws : h->pool) free_ws(ws);
   if (h->d_vec && h->vec_owned) cudaFree(h->d_vec);
+  if (h->d_codes) cudaFree(h->d_codes);
   if (h->d_vec64) cudaFree(h->d_vec64);
   if (h->d_adj0) cudaFree(h->d_adj0);
   if (h->d_upper_off) cudaFree(h->d_upper_off);

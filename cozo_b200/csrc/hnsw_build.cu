@@ -141,6 +141,7 @@ int hnsw_reserve(cozo_gpu_hnsw* h, uint32_t need_n, uint64_t need_up) {
       int rc = grow(h->d_vec, (size_t)h->cap_n * g.ld, (size_t)nc * g.ld, 0);
       if (rc) return rc;
     }
+    hnsw_codes_reserve(h, nc);
     int rc = grow(h->d_adj0, (size_t)h->cap_n * g.s0, (size_t)nc * g.s0, 0xFF);
     if (!rc) rc = grow(h->d_adj0_dist, (size_t)h->cap_n * g.s0, (size_t)nc * g.s0, 0);
     if (!rc) rc = grow(h->d_deg0, h->cap_n, nc, 0);
@@ -482,6 +483,7 @@ static int append_nodes(cozo_gpu_hnsw* h, const float* vectors, int on_device, u
   if (vectors)  // nullptr: the (borrowed) rows are already in place
     H_CUDA(cudaMemcpy2D(h->d_vec + (size_t)n0 * g.ld, (size_t)g.ld * 4, vectors, (size_t)g.dim * 4,
                         (size_t)g.dim * 4, count, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+  hnsw_codes_fill(h, n0, count);
   H_CUDA(cudaMemcpy(h->d_upper_off + n0, upper_off.data(), (size_t)count * 4, cudaMemcpyHostToDevice));
   H_CUDA(cudaMemcpy(h->d_node_level + n0, h->node_level.data() + n0, count, cudaMemcpyHostToDevice));
   if (!owners.empty())
@@ -514,6 +516,7 @@ extern "C" int cozo_gpu_hnsw_build(cozo_gpu_hnsw_t** out, const CozoGpuHnswBuild
   g.n = 0;
   g.dim = d->dim;
   g.ld = round_up(d->dim, 4);
+  g.code_ld = code_row_bytes(g.ld);
   g.metric = d->metric;
   g.entry = NONE;
   g.top_level = 0;
@@ -658,6 +661,7 @@ extern "C" int cozo_gpu_hnsw_update(cozo_gpu_hnsw_t* h, const uint32_t* ids, con
   uint32_t* d_ids = nullptr;
   H_CUDA(cudaMalloc(&d_ids, (size_t)count * 4));
   cudaMemcpy(d_ids, ids, (size_t)count * 4, cudaMemcpyHostToDevice);
+  hnsw_codes_fill(h, 0, count, d_ids);
   clear_dead_kernel<<<(count + 255) / 256, 256>>>(d_ids, count, h->d_dead);
   cudaError_t e = cudaDeviceSynchronize();
   cudaFree(d_ids);

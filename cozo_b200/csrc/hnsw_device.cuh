@@ -15,6 +15,7 @@
 //     cleared at the end of every layer through a log of the ids that were set.
 #pragma once
 #include "common.cuh"
+#include "hnsw_codes.cuh"
 
 namespace cozo {
 
@@ -29,6 +30,8 @@ struct HnswDev {
   uint32_t su;                // multiple of 32
   uint32_t entry;             // NONE = empty index
   uint32_t top_level;         // entry lives on layer -top_level
+  const uint8_t* codes;       // [n x code_ld] uint8 code rows (hnsw_codes.cuh); nullptr = no codes, nothing is pruned
+  uint32_t code_ld;           // bytes per code row
 };
 
 struct WarpCtx {
@@ -46,6 +49,11 @@ struct WarpCtx {
   uint32_t len, cursor, nlog;
   uint32_t head, phase;  // ring position / per-stage parity bits
   uint32_t dist_evals, nodes_expanded, nbr_reads;
+  uint32_t pruned;  // evaluations whose f32 row was never fetched (code_prune)
+  // code-row ring of the pruned search (used only when g.codes is set)
+  uint8_t* cring;
+  uint64_t* cbars;
+  uint32_t cns, chead, cphase;
 };
 
 constexpr uint32_t EXPANDED = 0x80000000u;
@@ -211,9 +219,85 @@ __device__ __forceinline__ void visit_clear(WarpCtx& w, int lane) {
   __syncwarp();
 }
 
+// f32 L2 distance from the query to a dequantised code row in shared memory, in dist_smem's lane-strided order.
+template <int NV>
+__device__ __forceinline__ float code_dist(const float4 (&q)[NV], const uint8_t* row, int lane, int nvec4) {
+  const float lo = reinterpret_cast<const float*>(row)[0];
+  const float scale = reinterpret_cast<const float*>(row)[1];
+  const uint32_t* c4 = reinterpret_cast<const uint32_t*>(row + CODE_HDR);
+  float a = 0.f, b = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    int idx = lane + 32 * i;
+    if (idx < nvec4) {
+      const uint32_t c = c4[idx];
+      float4 v;
+#if defined(__CUDA_ARCH__)
+      // byte k of c as an exact float: 2^23 + c_k with the exponent bits spliced in by PRMT, minus 2^23 (no I2F)
+      v.x = fmaf(__uint_as_float(__byte_perm(c, 0x4B000000u, 0x7650)) - 8388608.f, scale, lo);
+      v.y = fmaf(__uint_as_float(__byte_perm(c, 0x4B000000u, 0x7651)) - 8388608.f, scale, lo);
+      v.z = fmaf(__uint_as_float(__byte_perm(c, 0x4B000000u, 0x7652)) - 8388608.f, scale, lo);
+      v.w = fmaf(__uint_as_float(__byte_perm(c, 0x4B000000u, 0x7653)) - 8388608.f, scale, lo);
+#else
+      v.x = code_value(c & 0xFFu, lo, scale);
+      v.y = code_value((c >> 8) & 0xFFu, lo, scale);
+      v.z = code_value((c >> 16) & 0xFFu, lo, scale);
+      v.w = code_value(c >> 24, lo, scale);
+#endif
+      accum<COZO_GPU_L2>(q[i], v, a, b);
+    }
+  }
+  return warp_sum(a);
+}
+
+// Steps (a) and (b) of a pruned hop (L2, codes present, beam full): stream the code rows of the hop's `cnt` unvisited
+// neighbours w.pend[0..cnt) through the code ring, bound each one's distance from below (code_lower_bound) and keep,
+// in neighbour order, only those whose bound is below the beam's worst distance at the start of the hop.  While the
+// beam is full its last entry only decreases, so a neighbour dropped here would fail `d < fd[len-1]` too: nothing the
+// traversal does changes.  Returns the number of survivors, compacted to the front of w.pend.
+template <int NV>
+__device__ __forceinline__ uint32_t code_prune(const HnswDev& g, WarpCtx& w, const float4 (&q)[NV], uint32_t cnt,
+                                               int lane) {
+  const int nvec4 = g.ld >> 2;
+  const uint32_t crow = g.code_ld;
+  const double worst = (double)w.fd[w.len - 1];
+  uint32_t keep = 0;  // bit c: neighbour c survives
+  uint32_t issued = 0, si = w.chead, sc = w.chead;
+  for (uint32_t c = 0; c < cnt; ++c) {
+    if (lane == 0) {
+      fence_proxy_async_smem();
+      while (issued < cnt && issued - c < w.cns) {
+        mbar_expect_tx(&w.cbars[si], crow);
+        bulk_g2s(w.cring + (size_t)si * crow, g.codes + (size_t)w.pend[issued] * crow, crow, &w.cbars[si]);
+        ++issued;
+        if (++si == w.cns) si = 0;
+      }
+    }
+    mbar_wait(&w.cbars[sc], (w.cphase >> sc) & 1u);
+    w.cphase ^= (1u << sc);
+    const uint8_t* row = w.cring + (size_t)sc * crow;
+    const float dt = code_dist<NV>(q, row, lane, nvec4);
+    const float err = reinterpret_cast<const float*>(row)[2];
+    if (++sc == w.cns) sc = 0;
+    if (!(code_lower_bound(dt, err) >= worst)) keep |= 1u << c;
+    __syncwarp();  // every lane is done with the slot before lane 0 refills it
+  }
+  w.chead = sc;
+  const bool mine = (keep >> lane) & 1u;
+  const uint32_t id = mine ? w.pend[lane] : NONE;
+  __syncwarp();
+  if (mine) w.pend[__popc(keep & ((1u << lane) - 1))] = id;
+  __syncwarp();
+  const uint32_t kept = __popc(keep);
+  w.pruned += cnt - kept;
+  return kept;
+}
+
 // hnsw_search_level (hnsw.rs:539-587) for one query held in registers.
 // `level` 0 is the bottom layer.  On entry the sorted array holds found_nn.
-template <int NV, int METRIC, bool BULK>
+// PRUNE (L2 with the bulk ring): when g.codes is set, hops that start with a full beam first drop the neighbours that
+// code_prune proves cannot be admitted, then fetch f32 rows for the rest only.
+template <int NV, int METRIC, bool BULK, bool PRUNE = false>
 __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const float4 (&q)[NV], float qnorm,
                                              uint32_t ef, uint32_t level, int lane) {
   const int nvec4 = g.ld >> 2;
@@ -276,6 +360,7 @@ __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const
       if (isnew) w.pend[__popc(newmask & ((1u << lane) - 1))] = id;
       __syncwarp();
       w.dist_evals += cnt;
+      if (PRUNE && g.codes && w.len == ef && cnt) cnt = code_prune<NV>(g, w, q, cnt, lane);
       if (BULK) {
         // ring indices advance by compare-and-wrap (a runtime `% ns` costs ~20 instructions)
         uint32_t issued = 0, si = w.head, sc = w.head;
