@@ -90,6 +90,17 @@ __device__ __forceinline__ uint32_t emit_results(const SearchParams& p, const Wa
   return found;
 }
 
+#ifdef COZO_HOP_CLOCKS
+// tools/hop_clocks.py: the per-phase totals of every warp of the warp-per-query search since the last read
+__device__ unsigned long long g_hop_clocks[HC_N];
+extern "C" int cozo_gpu_hop_clocks(unsigned long long* out) {
+  COZO_CUDA(cudaMemcpyFromSymbol(out, g_hop_clocks, sizeof(g_hop_clocks)));
+  static const unsigned long long zero[HC_N] = {};
+  COZO_CUDA(cudaMemcpyToSymbol(g_hop_clocks, zero, sizeof(zero)));
+  return 0;
+}
+#endif
+
 // One warp per query, persistent CTAs pulling query indices from a counter.
 // MINB = resident CTAs per SM the register allocation is capped for (4 warps per CTA).
 template <int NV, int METRIC, bool BULK, int MINB>
@@ -119,6 +130,9 @@ __global__ void __launch_bounds__(128, MINB) hnsw_search_kernel(HnswDev g, Searc
   w.cns = p.cns;
   w.chead = 0;
   w.cphase = 0;
+#ifdef COZO_HOP_CLOCKS
+  for (int k = 0; k < HC_N; ++k) w.clk[k] = 0;
+#endif
   if (BULK) {
     if (lane == 0) {
       for (uint32_t s = 0; s < p.ns; ++s) mbar_init(&w.bars[s], 1);
@@ -167,6 +181,10 @@ __global__ void __launch_bounds__(128, MINB) hnsw_search_kernel(HnswDev g, Searc
     }
     __syncwarp();
   }
+#ifdef COZO_HOP_CLOCKS
+  if (lane == 0)
+    for (int k = 0; k < HC_N; ++k) atomicAdd(&g_hop_clocks[k], w.clk[k]);
+#endif
 }
 
 using KernelFn = void (*)(HnswDev, SearchParams);
@@ -510,8 +528,9 @@ int hnsw_launch_search(cozo_gpu_hnsw* h, HnswWorkspace* ws, const float* d_q, ui
     p.off_ring = round_up(p.off_bars + ns * 8, 128);
     p.warp_smem = round_up(p.off_ring + ns * g.ld * 4, 128);
     if (bulk && g.codes) {
-      // pruned search (code_prune): most rows of a hop never reach the f32 ring, so it keeps at most 2 stages and
+      // pruned search (prune_chunk): most rows of a hop never reach the f32 ring, so it keeps at most 2 stages and
       // the code ring takes the rest of the same per-warp budget; the CTAs resident per SM stay what they were.
+      // At config 2 (D = 768, ef 200) 1 f32 + 11 code stages and 2 + 7 measured within 0.5 % of each other.
       // [fd][fi][pend][bars ns][code bars <= 16][f32 ring ns][code ring cns]
       const uint32_t budget = p.warp_smem;
       ns = std::min<uint32_t>(ns, 2);

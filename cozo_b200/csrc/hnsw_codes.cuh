@@ -18,8 +18,11 @@ namespace cozo {
 constexpr uint32_t CODE_HDR = 16;
 // Only rows of at least this many elements get codes.  Pruning trades a second, dependent fetch per hop for fewer
 // bytes: at D = 768 (3 KB rows) a step is 1.5x faster, at D = 128 (512 B rows, latency-bound) it was 13 % slower
-// (one H100, bench.py config 2 and --dim 128); dims in between are not measured.
-constexpr uint32_t CODES_MIN_LD = 512;
+// (one H100, bench.py config 2 and --dim 128); dims in between are not measured.  Overridable so that the CPU emulator
+// of the library can run the pruned search at small dimensions.
+#ifndef CODES_MIN_LD
+#define CODES_MIN_LD 512u
+#endif
 
 __host__ __device__ inline uint32_t code_row_bytes(uint32_t ld) { return CODE_HDR + (ld + 15) / 16 * 16; }
 
@@ -75,12 +78,24 @@ __host__ __device__ inline void quantize_row(const float* x, uint32_t ld, uint8_
 //   most 2^-17 relative for ld <= 2048.  REL = 2^-14 covers both sides with room to spare; the absolute 1e-36
 //   covers subnormal underflow (< 2^-140 over the whole sum).  The f64 steps below round at 2^-53.
 // A distance that is NaN or overflowed gives no bound (0).  Prune only when the bound is >= the beam's worst.
+constexpr double CODE_REL = 0x1p-14;
 __host__ __device__ inline double code_lower_bound(float dt, float err) {
-  const double REL = 0x1p-14;
   if (!(dt <= 3.40282347e38f)) return 0.0;
-  const double s = sqrt((double)dt * (1.0 - REL)) - (double)err;
+  const double s = sqrt((double)dt * (1.0 - CODE_REL)) - (double)err;
   if (!(s > 0.0)) return 0.0;
-  return s * s * (1.0 - REL) - 1e-36;
+  return s * s * (1.0 - CODE_REL) - 1e-36;
+}
+
+// The same test without a square root per row: code_lower_bound(dt, err) >= worst  <=>  s >= W with
+// W = sqrt((worst + 1e-36) / (1 - REL))  <=>  dt (1 - REL) >= (err + W)^2, all in exact arithmetic.  W depends only on the
+// beam's worst distance, so the search computes it once per value of worst (code_prune_radius) and tests each row with
+// code_prunes.  Rounding: the f64 steps here round at 2^-53, far inside the 2^-14 - 2^-17 margin that REL leaves over the
+// f32 error of d and dt, so pruning still implies d >= worst.  A NaN or overflowed dt, err = +inf, or a NaN or +inf
+// worst never prunes.
+__host__ __device__ inline double code_prune_radius(float worst) { return sqrt(((double)worst + 1e-36) / (1.0 - CODE_REL)); }
+__host__ __device__ inline bool code_prunes(float dt, float err, double W) {
+  const double r = (double)err + W;
+  return dt <= 3.40282347e38f && (double)dt * (1.0 - CODE_REL) >= r * r;
 }
 
 // Fills the code rows of vectors ids[i] (ids == nullptr: first + i) for i < count.  One thread per row: this runs

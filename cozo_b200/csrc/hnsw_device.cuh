@@ -34,6 +34,19 @@ struct HnswDev {
   uint32_t code_ld;           // bytes per code row
 };
 
+// Per-phase clock64 totals of the warp-per-query search, compiled only with -DCOZO_HOP_CLOCKS (tools/hop_clocks.py):
+// pop + adjacency read, visited test, code-ring waits, code scoring, f32-ring waits, f32 scoring + admissions.
+enum HopPhase { HC_POP, HC_VISIT, HC_CWAIT, HC_CSCORE, HC_FWAIT, HC_FSCORE, HC_N };
+#ifdef COZO_HOP_CLOCKS
+#define HOP_T(t) long long t = clock64()
+#define HOP_SET(t) (t = clock64())
+#define HOP_ADD(w, k, t) ((w).clk[k] += (unsigned long long)(clock64() - (t)))
+#else
+#define HOP_T(t)
+#define HOP_SET(t)
+#define HOP_ADD(w, k, t)
+#endif
+
 struct WarpCtx {
   float* fd;       // smem: sorted distances (ascending)
   uint32_t* fi;    // smem: ids, bit31 = expanded
@@ -49,11 +62,14 @@ struct WarpCtx {
   uint32_t len, cursor, nlog;
   uint32_t head, phase;  // ring position / per-stage parity bits
   uint32_t dist_evals, nodes_expanded, nbr_reads;
-  uint32_t pruned;  // evaluations whose f32 row was never fetched (code_prune)
+  uint32_t pruned;  // evaluations whose f32 row was never fetched (prune_chunk)
   // code-row ring of the pruned search (used only when g.codes is set)
   uint8_t* cring;
   uint64_t* cbars;
   uint32_t cns, chead, cphase;
+#ifdef COZO_HOP_CLOCKS
+  unsigned long long clk[HC_N];
+#endif
 };
 
 constexpr uint32_t EXPANDED = 0x80000000u;
@@ -102,6 +118,25 @@ __device__ __forceinline__ float dist_smem(const float4 (&q)[NV], const float4* 
     if (idx < nvec4) accum<METRIC>(q[i], row[idx], a, b);
   }
   return finish<METRIC>(a, b, qnorm);
+}
+
+// dist_smem's L2 distance (same order, same result) with every shared-memory load issued before the first FMA, for the
+// pruned search; dist_smem itself stays as the other kernels use it.
+template <int NV>
+__device__ __forceinline__ float dist_smem_l2(const float4 (&q)[NV], const float4* row, int lane, int nvec4) {
+  float4 v[NV];
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    int idx = lane + 32 * i;
+    if (idx < nvec4) v[i] = row[idx];
+  }
+  float a = 0.f, b = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    int idx = lane + 32 * i;
+    if (idx < nvec4) accum<COZO_GPU_L2>(q[i], v[i], a, b);
+  }
+  return finish<COZO_GPU_L2>(a, b, 0.f);
 }
 
 // two rows at once straight from HBM: all 2*NV 128-bit loads are issued before
@@ -219,84 +254,208 @@ __device__ __forceinline__ void visit_clear(WarpCtx& w, int lane) {
   __syncwarp();
 }
 
-// f32 L2 distance from the query to a dequantised code row in shared memory, in dist_smem's lane-strided order.
+// f32 L2 distances from the query to two dequantised code rows in shared memory, each in dist_smem's lane-strided order
+// (the order codes_bound_emu.cpp checks the bound in).  The two FMA chains and shuffle trees are independent, so one
+// warp keeps twice the work in flight.
 template <int NV>
-__device__ __forceinline__ float code_dist(const float4 (&q)[NV], const uint8_t* row, int lane, int nvec4) {
-  const float lo = reinterpret_cast<const float*>(row)[0];
-  const float scale = reinterpret_cast<const float*>(row)[1];
-  const uint32_t* c4 = reinterpret_cast<const uint32_t*>(row + CODE_HDR);
-  float a = 0.f, b = 0.f;
+__device__ __forceinline__ void code_dist2(const float4 (&q)[NV], const uint8_t* r0, const uint8_t* r1, int lane,
+                                           int nvec4, float& d0, float& d1) {
+  const float lo0 = reinterpret_cast<const float*>(r0)[0], scale0 = reinterpret_cast<const float*>(r0)[1];
+  const float lo1 = reinterpret_cast<const float*>(r1)[0], scale1 = reinterpret_cast<const float*>(r1)[1];
+  const uint32_t* c0 = reinterpret_cast<const uint32_t*>(r0 + CODE_HDR);
+  const uint32_t* c1 = reinterpret_cast<const uint32_t*>(r1 + CODE_HDR);
+  // every shared-memory load first, so their latencies overlap (above NV = 8 that needs more registers than the
+  // kernel has: loaded where used)
+  constexpr bool HOIST = NV <= 8;
+  uint32_t w0[NV], w1[NV];
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    int idx = lane + 32 * i;
+    if (HOIST) {
+      w0[i] = idx < nvec4 ? c0[idx] : 0u;
+      w1[i] = idx < nvec4 ? c1[idx] : 0u;
+    }
+  }
+  float a0 = 0.f, a1 = 0.f, b = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     int idx = lane + 32 * i;
     if (idx < nvec4) {
-      const uint32_t c = c4[idx];
-      float4 v;
+      const uint32_t u0 = HOIST ? w0[i] : c0[idx], u1 = HOIST ? w1[i] : c1[idx];
+      float4 v0, v1;
 #if defined(__CUDA_ARCH__)
-      // byte k of c as an exact float: 2^23 + c_k with the exponent bits spliced in by PRMT, minus 2^23 (no I2F)
-      v.x = fmaf(__uint_as_float(__byte_perm(c, 0x4B000000u, 0x7650)) - 8388608.f, scale, lo);
-      v.y = fmaf(__uint_as_float(__byte_perm(c, 0x4B000000u, 0x7651)) - 8388608.f, scale, lo);
-      v.z = fmaf(__uint_as_float(__byte_perm(c, 0x4B000000u, 0x7652)) - 8388608.f, scale, lo);
-      v.w = fmaf(__uint_as_float(__byte_perm(c, 0x4B000000u, 0x7653)) - 8388608.f, scale, lo);
+      // byte k of u as an exact float: 2^23 + u_k with the exponent bits spliced in by PRMT, minus 2^23 (no I2F)
+      v0.x = fmaf(__uint_as_float(__byte_perm(u0, 0x4B000000u, 0x7650)) - 8388608.f, scale0, lo0);
+      v0.y = fmaf(__uint_as_float(__byte_perm(u0, 0x4B000000u, 0x7651)) - 8388608.f, scale0, lo0);
+      v0.z = fmaf(__uint_as_float(__byte_perm(u0, 0x4B000000u, 0x7652)) - 8388608.f, scale0, lo0);
+      v0.w = fmaf(__uint_as_float(__byte_perm(u0, 0x4B000000u, 0x7653)) - 8388608.f, scale0, lo0);
+      v1.x = fmaf(__uint_as_float(__byte_perm(u1, 0x4B000000u, 0x7650)) - 8388608.f, scale1, lo1);
+      v1.y = fmaf(__uint_as_float(__byte_perm(u1, 0x4B000000u, 0x7651)) - 8388608.f, scale1, lo1);
+      v1.z = fmaf(__uint_as_float(__byte_perm(u1, 0x4B000000u, 0x7652)) - 8388608.f, scale1, lo1);
+      v1.w = fmaf(__uint_as_float(__byte_perm(u1, 0x4B000000u, 0x7653)) - 8388608.f, scale1, lo1);
 #else
-      v.x = code_value(c & 0xFFu, lo, scale);
-      v.y = code_value((c >> 8) & 0xFFu, lo, scale);
-      v.z = code_value((c >> 16) & 0xFFu, lo, scale);
-      v.w = code_value(c >> 24, lo, scale);
+      v0.x = code_value(u0 & 0xFFu, lo0, scale0);
+      v0.y = code_value((u0 >> 8) & 0xFFu, lo0, scale0);
+      v0.z = code_value((u0 >> 16) & 0xFFu, lo0, scale0);
+      v0.w = code_value(u0 >> 24, lo0, scale0);
+      v1.x = code_value(u1 & 0xFFu, lo1, scale1);
+      v1.y = code_value((u1 >> 8) & 0xFFu, lo1, scale1);
+      v1.z = code_value((u1 >> 16) & 0xFFu, lo1, scale1);
+      v1.w = code_value(u1 >> 24, lo1, scale1);
 #endif
-      accum<COZO_GPU_L2>(q[i], v, a, b);
+      accum<COZO_GPU_L2>(q[i], v0, a0, b);
+      accum<COZO_GPU_L2>(q[i], v1, a1, b);
     }
   }
-  return warp_sum(a);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    a0 += __shfl_xor_sync(0xffffffffu, a0, o);
+    a1 += __shfl_xor_sync(0xffffffffu, a1, o);
+  }
+  d0 = a0;
+  d1 = a1;
 }
 
-// Steps (a) and (b) of a pruned hop (L2, codes present, beam full): stream the code rows of the hop's `cnt` unvisited
-// neighbours w.pend[0..cnt) through the code ring, bound each one's distance from below (code_lower_bound) and keep,
-// in neighbour order, only those whose bound is below the beam's worst distance at the start of the hop.  While the
-// beam is full its last entry only decreases, so a neighbour dropped here would fail `d < fd[len-1]` too: nothing the
-// traversal does changes.  Returns the number of survivors, compacted to the front of w.pend.
+// One 32-id adjacency chunk of a pruned hop (L2, codes present, beam full), as one stream per warp.  `id` is this lane's
+// neighbour id (NONE = idle), `validmask` the lanes that hold one.
+//   * The code rows of the first w.cns valid ids are issued before the visited test, so their fetch overlaps the
+//     atomicOr round trip.  Those that turn out to be visited are waited for and discarded (not scored, not counted);
+//     later ids are fetched only if they are unvisited.  Stream position p holds w.pend[p], bit 31 set = discard.
+//   * Each code row is bounded from below (hnsw_codes.cuh) against the beam's worst distance AT THAT MOMENT.  With a
+//     full beam fd[len-1] only decreases, and a neighbour's admission test `d < fd[len-1]` comes after every earlier
+//     survivor's admission, so the value tested here is at least the one its admission would face: a dropped
+//     neighbour could not have been admitted.
+//   * A survivor's f32 row is issued as soon as an f32 slot is free and consumed, in survivor (= neighbour) order,
+//     as soon as it has landed (polled, never waited for while code rows remain); the rest are drained at the end.
+//     Admissions therefore happen in neighbour order with the live bound, exactly as without pruning: ids, distances
+//     and the traversal counters are unchanged; only the number of f32 rows fetched can go down.
 template <int NV>
-__device__ __forceinline__ uint32_t code_prune(const HnswDev& g, WarpCtx& w, const float4 (&q)[NV], uint32_t cnt,
-                                               int lane) {
+__device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const float4 (&q)[NV], uint32_t ef,
+                                            uint32_t id, uint32_t validmask, int lane) {
   const int nvec4 = g.ld >> 2;
-  const uint32_t crow = g.code_ld;
-  const double worst = (double)w.fd[w.len - 1];
-  uint32_t keep = 0;  // bit c: neighbour c survives
-  uint32_t issued = 0, si = w.chead, sc = w.chead;
-  for (uint32_t c = 0; c < cnt; ++c) {
-    if (lane == 0) {
+  const uint32_t crow = g.code_ld, row_bytes = g.ld * 4;
+  const uint32_t lt = (1u << lane) - 1;
+  const uint32_t rank = __popc(validmask & lt);
+  const uint32_t spec = min((uint32_t)__popc(validmask), w.cns);  // speculative code rows: valid ids of rank < spec
+  const bool early = id != NONE && rank < spec;
+  HOP_T(t0);
+  if (early) {
+    uint32_t s = w.chead + rank;
+    if (s >= w.cns) s -= w.cns;
+    fence_proxy_async_smem();
+    mbar_expect_tx(&w.cbars[s], crow);
+    bulk_g2s(w.cring + (size_t)s * crow, g.codes + (size_t)id * crow, crow, &w.cbars[s]);
+  }
+  uint32_t newmask;
+  const bool isnew = visit_mark(w, id, lane, newmask);  // hnsw.rs:569-571,582
+  const uint32_t earlymask = __ballot_sync(0xffffffffu, early);
+  w.dist_evals += __popc(newmask);
+  if (early) w.pend[rank] = isnew ? id : id | EXPANDED;
+  else if (isnew) w.pend[spec + __popc(newmask & ~earlymask & lt)] = id;
+  const uint32_t len = spec + __popc(newmask & ~earlymask);
+  __syncwarp();
+  HOP_ADD(w, HC_VISIT, t0);
+
+  uint32_t fq = 0, fin = 0;  // bits by stream position: survivors whose f32 row is queued / in flight (in order)
+  double W = code_prune_radius(w.fd[ef - 1]);
+  // f32 ring: slot w.head holds the oldest row in flight, popc(fin) rows are in flight
+  auto f32_issue = [&]() {
+    while (fq && __popc(fin) < w.ns) {
+      const uint32_t c = __ffs(fq) - 1;
+      if (lane == 0) {
+        uint32_t s = w.head + __popc(fin);
+        if (s >= w.ns) s -= w.ns;
+        fence_proxy_async_smem();
+        mbar_expect_tx(&w.bars[s], row_bytes);
+        bulk_g2s(w.ring + (size_t)s * g.ld, g.vec + (size_t)w.pend[c] * g.ld, row_bytes, &w.bars[s]);
+      }
+      fq &= fq - 1;
+      fin |= 1u << c;
+    }
+  };
+  auto f32_consume = [&]() {
+    HOP_T(t1);
+    mbar_wait(&w.bars[w.head], (w.phase >> w.head) & 1u);
+    w.phase ^= (1u << w.head);
+    HOP_ADD(w, HC_FWAIT, t1);
+    HOP_T(t2);
+    const float4* row = reinterpret_cast<const float4*>(w.ring + (size_t)w.head * g.ld);
+    // above NV = 6 the loads-first form needs more registers than the kernel has (it spills)
+    const float d = NV > 6 ? dist_smem<NV, COZO_GPU_L2>(q, row, lane, nvec4, 0.f) : dist_smem_l2<NV>(q, row, lane, nvec4);
+    if (++w.head == w.ns) w.head = 0;
+    const uint32_t nid = w.pend[__ffs(fin) - 1];
+    fin &= fin - 1;
+    __syncwarp();
+    if (d < w.fd[ef - 1]) {  // hnsw.rs:575-581 (the beam stays full)
+      sorted_insert(w, ef, d, nid, lane);
+      W = code_prune_radius(w.fd[ef - 1]);
+    }
+    HOP_ADD(w, HC_FSCORE, t2);
+  };
+
+  // code rows two at a time (code_dist2); position `issued` is the next one to fetch, into slot chead + issued - c
+  uint32_t issued = spec;
+  for (uint32_t c = 0; c < len;) {
+    const uint32_t upto = min(len, c + w.cns);
+    if (lane == 0 && issued < upto) {
       fence_proxy_async_smem();
-      while (issued < cnt && issued - c < w.cns) {
-        mbar_expect_tx(&w.cbars[si], crow);
-        bulk_g2s(w.cring + (size_t)si * crow, g.codes + (size_t)w.pend[issued] * crow, crow, &w.cbars[si]);
-        ++issued;
-        if (++si == w.cns) si = 0;
+      for (uint32_t p = issued; p < upto; ++p) {
+        uint32_t s = w.chead + (p - c);
+        if (s >= w.cns) s -= w.cns;
+        mbar_expect_tx(&w.cbars[s], crow);
+        bulk_g2s(w.cring + (size_t)s * crow, g.codes + (size_t)w.pend[p] * crow, crow, &w.cbars[s]);
       }
     }
-    mbar_wait(&w.cbars[sc], (w.cphase >> sc) & 1u);
-    w.cphase ^= (1u << sc);
-    const uint8_t* row = w.cring + (size_t)sc * crow;
-    const float dt = code_dist<NV>(q, row, lane, nvec4);
-    const float err = reinterpret_cast<const float*>(row)[2];
-    if (++sc == w.cns) sc = 0;
-    if (!(code_lower_bound(dt, err) >= worst)) keep |= 1u << c;
-    __syncwarp();  // every lane is done with the slot before lane 0 refills it
+    issued = max(issued, upto);
+    const bool two = c + 1 < len;
+    uint32_t s1 = w.chead + 1;
+    if (s1 == w.cns) s1 = 0;
+    HOP_T(t3);
+    mbar_wait(&w.cbars[w.chead], (w.cphase >> w.chead) & 1u);
+    w.cphase ^= (1u << w.chead);
+    if (two) {
+      mbar_wait(&w.cbars[s1], (w.cphase >> s1) & 1u);
+      w.cphase ^= (1u << s1);
+    }
+    HOP_ADD(w, HC_CWAIT, t3);
+    HOP_T(t4);
+    const uint8_t* r0 = w.cring + (size_t)w.chead * crow;
+    const uint8_t* r1 = two ? w.cring + (size_t)s1 * crow : r0;
+    float dt0, dt1;
+    code_dist2<NV>(q, r0, r1, lane, nvec4, dt0, dt1);
+    const float err0 = reinterpret_cast<const float*>(r0)[2], err1 = reinterpret_cast<const float*>(r1)[2];
+    const uint32_t p0 = w.pend[c], p1 = two ? w.pend[c + 1] : EXPANDED;
+    __syncwarp();  // every lane is done with the two slots before lane 0 refills them
+    if (!(p0 & EXPANDED)) {
+      if (code_prunes(dt0, err0, W)) w.pruned++;
+      else fq |= 1u << c;
+    }
+    if (!(p1 & EXPANDED)) {
+      if (code_prunes(dt1, err1, W)) w.pruned++;
+      else fq |= 1u << (c + 1);
+    }
+    const uint32_t step = two ? 2 : 1;
+    w.chead += step;
+    if (w.chead >= w.cns) w.chead -= w.cns;
+    c += step;
+    HOP_ADD(w, HC_CSCORE, t4);
+    f32_issue();
+    // admit the rows that have landed; a row in flight is not waited for while code rows remain
+    while (fin && __shfl_sync(0xffffffffu, lane == 0 ? (uint32_t)mbar_try_wait(&w.bars[w.head], (w.phase >> w.head) & 1u) : 0u, 0)) {
+      f32_consume();
+      f32_issue();
+    }
   }
-  w.chead = sc;
-  const bool mine = (keep >> lane) & 1u;
-  const uint32_t id = mine ? w.pend[lane] : NONE;
-  __syncwarp();
-  if (mine) w.pend[__popc(keep & ((1u << lane) - 1))] = id;
-  __syncwarp();
-  const uint32_t kept = __popc(keep);
-  w.pruned += cnt - kept;
-  return kept;
+  while (fin) {
+    f32_consume();
+    f32_issue();
+  }
 }
 
 // hnsw_search_level (hnsw.rs:539-587) for one query held in registers.
 // `level` 0 is the bottom layer.  On entry the sorted array holds found_nn.
-// PRUNE (L2 with the bulk ring): when g.codes is set, hops that start with a full beam first drop the neighbours that
-// code_prune proves cannot be admitted, then fetch f32 rows for the rest only.
+// PRUNE (L2 with the bulk ring): when g.codes is set, the chunks of a hop that find the beam full run prune_chunk, which
+// fetches f32 rows only for the neighbours whose code row cannot rule out admission.
 template <int NV, int METRIC, bool BULK, bool PRUNE = false>
 __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const float4 (&q)[NV], float qnorm,
                                              uint32_t ef, uint32_t level, int lane) {
@@ -318,6 +477,7 @@ __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const
   const uint32_t stride = level == 0 ? g.s0 : g.su;
 
   for (;;) {
+    HOP_T(tp);
     // candidates.pop(): nearest not-yet-expanded entry (hnsw.rs:559)
     uint32_t ci = NONE;
     for (uint32_t base = w.cursor & ~31u; base < w.len; base += 32) {
@@ -350,17 +510,25 @@ __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const
       row = g.adj_up + (size_t)(off + level - 1) * g.su;
     }
     for (uint32_t nb = 0; nb < stride; nb += 32) {
+      if (nb) HOP_SET(tp);
       uint32_t id = __ldg(row + nb + lane);
       uint32_t validmask = __ballot_sync(0xffffffffu, id != NONE);
+      HOP_ADD(w, HC_POP, tp);
       if (!validmask) break;
       w.nbr_reads += __popc(validmask);
+      if (PRUNE && g.codes && w.len == ef) {
+        prune_chunk<NV>(g, w, q, ef, id, validmask, lane);
+        __syncwarp();
+        continue;
+      }
+      HOP_T(tv);
       uint32_t newmask;
       bool isnew = visit_mark(w, id, lane, newmask);  // hnsw.rs:569-571,582
       uint32_t cnt = __popc(newmask);
       if (isnew) w.pend[__popc(newmask & ((1u << lane) - 1))] = id;
       __syncwarp();
+      HOP_ADD(w, HC_VISIT, tv);
       w.dist_evals += cnt;
-      if (PRUNE && g.codes && w.len == ef && cnt) cnt = code_prune<NV>(g, w, q, cnt, lane);
       if (BULK) {
         // ring indices advance by compare-and-wrap (a runtime `% ns` costs ~20 instructions)
         uint32_t issued = 0, si = w.head, sc = w.head;
@@ -374,14 +542,18 @@ __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const
               if (++si == w.ns) si = 0;
             }
           }
+          HOP_T(tw);
           mbar_wait(&w.bars[sc], (w.phase >> sc) & 1u);
           w.phase ^= (1u << sc);
+          HOP_ADD(w, HC_FWAIT, tw);
+          HOP_T(ts);
           float d = dist_smem<NV, METRIC>(q, reinterpret_cast<const float4*>(w.ring + (size_t)sc * g.ld), lane, nvec4,
                                           qnorm);
           if (++sc == w.ns) sc = 0;
           uint32_t nid = w.pend[c];
           __syncwarp();
           if (w.len < ef || d < w.fd[w.len - 1]) sorted_insert(w, ef, d, nid, lane);  // hnsw.rs:575-581
+          HOP_ADD(w, HC_FSCORE, ts);
         }
         w.head = sc;
       } else {
