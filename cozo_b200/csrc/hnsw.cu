@@ -36,6 +36,7 @@ struct SearchParams {
   uint32_t n_dest, slot;
   uint32_t* dest_ids[COZO_GPU_MAX_PEERS];
   float* dest_dist[COZO_GPU_MAX_PEERS];
+  uint32_t off_qcodes;  // the pruned search's fixed-point query (QueryCodes::a)
 };
 
 
@@ -152,6 +153,9 @@ __global__ void __launch_bounds__(128, MINB) hnsw_search_kernel(HnswDev g, Searc
     float4 q[NV];
     float qnorm;
     load_query<NV>(p.queries + (size_t)qi * g.dim, g.dim, lane, q, qnorm);
+    QueryCodes qc;
+    qc.a = reinterpret_cast<QueryPair*>(base + p.off_qcodes);
+    if (PRUNE && g.codes) load_query_codes<NV>(q, g.ld, lane, qc);
     w.len = 0;
     w.cursor = 0;
     w.dist_evals = w.nodes_expanded = w.nbr_reads = w.pruned = 0;
@@ -168,8 +172,8 @@ __global__ void __launch_bounds__(128, MINB) hnsw_search_kernel(HnswDev g, Searc
       w.len = 1;
       __syncwarp();
       for (uint32_t lvl = g.top_level; lvl >= 1; --lvl)  // hnsw.rs:919-929
-        search_level<NV, METRIC, BULK, PRUNE>(g, w, q, qnorm, 1, lvl, lane);
-      search_level<NV, METRIC, BULK, PRUNE>(g, w, q, qnorm, p.ef, 0, lane);  // hnsw.rs:930-938
+        search_level<NV, METRIC, BULK, PRUNE>(g, w, q, qnorm, 1, lvl, lane, &qc);
+      search_level<NV, METRIC, BULK, PRUNE>(g, w, q, qnorm, p.ef, 0, lane, &qc);  // hnsw.rs:930-938
     }
     found = emit_results(p, w, qi, lane, g.entry != NONE);
     if (lane == 0) {
@@ -530,12 +534,15 @@ int hnsw_launch_search(cozo_gpu_hnsw* h, HnswWorkspace* ws, const float* d_q, ui
     if (bulk && g.codes) {
       // pruned search (prune_chunk): most rows of a hop never reach the f32 ring, so it keeps at most 2 stages and
       // the code ring takes the rest of the same per-warp budget; the CTAs resident per SM stay what they were.
-      // At config 2 (D = 768, ef 200) 1 f32 + 11 code stages and 2 + 7 measured within 0.5 % of each other.
-      // [fd][fi][pend][bars ns][code bars <= 16][f32 ring ns][code ring cns]
+      // The fixed-point query (QueryCodes, 256 B per 128 elements) is taken from the code ring: at config 2 (D = 768,
+      // ef 200) that leaves 2 f32 + 5 code stages (7 before); hnsw.stages=1 (1 + 2) measured 0.9 % slower
+      // (tools/sweep.py).
+      // [fd][fi][pend][bars ns][code bars <= 16][fixed-point query][f32 ring ns][code ring cns]
       const uint32_t budget = p.warp_smem;
       ns = std::min<uint32_t>(ns, 2);
       p.off_cbars = p.off_bars + ns * 8;
-      p.off_ring = round_up(p.off_cbars + 16 * 8, 128);
+      p.off_qcodes = p.off_cbars + 16 * 8;
+      p.off_ring = round_up(p.off_qcodes + (g.ld / 4 + 31) / 32 * 256, 128);
       p.off_cring = p.off_ring + ns * g.ld * 4;  // a multiple of 16: ld is a multiple of 4
       const uint32_t room = budget > p.off_cring ? budget - p.off_cring : 0;
       p.cns = std::min<uint32_t>(16, std::max<uint32_t>(2, room / g.code_ld));

@@ -3,11 +3,12 @@
 //
 // Layout: one code row per vector, code_row_bytes(ld) = 16 + round_up(ld, 16) bytes, so that a row is one
 // cp.async.bulk (16-byte aligned, a multiple of 16 bytes long):
-//   float lo, scale, err, 0      the row header
+//   float lo, scale, err, X2     the row header
 //   uint8 c[ld]                  one code per element of the f32 row, padding elements included; zero padded
-// Element j dequantises to  x~_j = fmaf((float)c_j, scale, lo)  (code_value), which is exactly what the search
-// computes.  err >= ||x - x~||_2 over all ld elements, computed in f64 from those very f32 values and rounded up;
-// a row holding NaN or +-inf (or whose range overflows f32) gets err = +inf and is never pruned.
+// Element j dequantises to  x~_j = fmaf((float)c_j, scale, lo)  (code_value), and in exact arithmetic to
+// x^_j = lo + scale c_j.  err >= ||x - x~||_2 and err >= ||x - x^||_2 over all ld elements, computed in f64 and rounded
+// up; X2 <= ||x^||^2, computed in f64 and rounded down.  A row holding NaN or +-inf (or whose range or X2 overflows f32)
+// gets err = +inf and is never pruned.
 #pragma once
 #include <math.h>
 
@@ -44,7 +45,7 @@ __host__ __device__ inline void quantize_row(const float* x, uint32_t ld, uint8_
   if (!code_finite(scale)) finite = false;
   if (!finite) lo = scale = 0.f;
   uint8_t* c = out + CODE_HDR;
-  double ss = 0.0;
+  double ss = 0.0, x2 = 0.0;
   for (uint32_t j = 0; j < ld; ++j) {
     uint32_t cj = 0;
     if (scale > 0.f) {
@@ -52,22 +53,35 @@ __host__ __device__ inline void quantize_row(const float* x, uint32_t ld, uint8_
       cj = t > 0.f ? (t < 255.f ? (uint32_t)t : 255u) : 0u;
     }
     c[j] = (uint8_t)cj;
-    const double e = (double)x[j] - (double)code_value(cj, lo, scale);
+    // |x - x^| <= |x - x~| + |x~ - x^|, and x~ - x^ is the rounding of one fmaf: at most half an ulp of x~, which is
+    // <= 2^-24 |x~| + 2^-150; none when c = 0 (x~ = x^ = lo)
+    const float xt = code_value(cj, lo, scale);
+    const double e = fabs((double)x[j] - (double)xt) + (cj ? fabs((double)xt) * 0x1p-24 + 0x1p-150 : 0.0);
     ss += e * e;
+    const double xe = fma((double)scale, (double)cj, (double)lo);
+    x2 += xe * xe;
   }
   for (uint32_t j = ld; j < code_row_bytes(ld) - CODE_HDR; ++j) c[j] = 0;
-  // ss carries at most (2 ld + 2) f64 roundings, far below the 2^-30 the two factors add
-  float err = INFINITY;
+  // ss and x2 are sums of non-negative terms and carry at most (2 ld + 6) f64 roundings, far below the 2^-30 the
+  // factors add
+  float err = INFINITY, X2 = 0.f;
   if (finite) {
     const double e = sqrt(ss * (1.0 + 0x1p-30)) * (1.0 + 0x1p-30);
     err = (float)e;
     if ((double)err < e) err = nextafterf(err, INFINITY);
+    const double xl = x2 * (1.0 - 0x1p-30);
+    X2 = (float)xl;
+    if ((double)X2 > xl) X2 = nextafterf(X2, 0.f);
+    if (!code_finite(X2)) {
+      err = INFINITY;
+      X2 = 0.f;
+    }
   }
   float* hdr = reinterpret_cast<float*>(out);
   hdr[0] = lo;
   hdr[1] = scale;
   hdr[2] = err;
-  hdr[3] = 0.f;
+  hdr[3] = X2;
 }
 
 // Lower bound on the search kernel's f32 L2 distance d(q, x), from dt = the kernel's f32 distance to the
@@ -96,6 +110,99 @@ __host__ __device__ inline double code_prune_radius(float worst) { return sqrt((
 __host__ __device__ inline bool code_prunes(float dt, float err, double W) {
   const double r = (double)err + W;
   return dt <= 3.40282347e38f && (double)dt * (1.0 - CODE_REL) >= r * r;
+}
+
+// ---- the integer form of the bound: what the search runs ------------------------------------------------------------
+// The query is held in fixed point, q^_j = s_q a_j with integers |a_j| <= A = code_query_amax(ld), so that the exact
+// integer S = sum_j a_j c_j fits in an int32 over the whole row (|S| <= A 255 ld < 2^31, and so does every partial sum).
+// s_q is a power of two, the least one with max_j |q_j| <= A s_q, so q_j - s_q a_j is exact in f64.
+// With e_q >= ||q - q^|| (per query) and err >= ||x - x^|| (per row), the triangle inequality twice gives
+//   ||q - x|| >= ||q^ - x^|| - e_q - err,    ||q^ - x^||^2 = D^ = Q2 + ||x^||^2 - 2 s_q (lo sum_j a_j + scale S)
+// with Q2 = s_q^2 sum_j a_j^2 (exact in f64).  The search evaluates D^ in f64 with the row's X2 <= ||x^||^2 in place of
+// ||x^||^2 (only lowering it) and subtracts 2^-45 (Q2 + X2 + 2 s_q (|lo sum a| + |scale S|)), which covers the f64
+// roundings of the expansion (under 2^-50 of that sum).  The result D^_lo <= D^ prunes iff D^_lo >= (err + e_q + W)^2
+// with W = code_prune_radius(worst): then sqrt(D) >= W, and the REL argument of code_prunes gives d >= worst.  The f64
+// roundings of err + e_q + W and of its square are relative to err, e_q and W, and the 2^-30 on err and e_q and the
+// REL on W cover them.  Nothing prunes when D^_lo, err or e_q is NaN or +inf; a query holding NaN or +-inf has e_q = +inf.
+// Tightness: X2 is rounded to f32, so on rows whose offset dwarfs their spread (|lo| >> scale) D^_lo falls short of D^
+// by up to 2^-24 ||x^||^2 and those rows prune less often; the bound stays valid.
+struct CodeQuery {
+  double q2;     // ||q^||^2 = s_q^2 sum a_j^2
+  double sq2;    // 2 s_q
+  int32_t suma;  // sum a_j
+  double eq;     // >= ||q - q^||; +inf: nothing is pruned
+};
+
+__host__ __device__ inline int32_t code_query_amax(uint32_t ld) {
+  const uint32_t a = 2147483647u / (255u * (ld ? ld : 1u));
+  return (int32_t)(a < 32767u ? a : 32767u);
+}
+
+// s_q for a query whose largest |q_j| is m (finite): the least power of two with m <= A s_q (1 if m = 0)
+__host__ __device__ inline double code_query_scale(float m, int32_t A) {
+  if (!(m > 0.f)) return 1.0;
+  int e;
+  frexp((double)m / (double)A, &e);  // m / A < 2^e, up to the rounding of the division, which the clamp below absorbs
+  return ldexp(1.0, e);
+}
+
+// a_j for q_j (any value: the clamp keeps |a_j| <= A; a NaN maps to 0 and is caught by e_q)
+__host__ __device__ inline int32_t code_query_level(float q, double sq, int32_t A) {
+  const double t = rint((double)q / sq);
+  if (t >= (double)A) return A;
+  if (t <= -(double)A) return -A;
+  return t == t ? (int32_t)t : 0;
+}
+
+// the square of q_j - s_q a_j (exact before squaring: both are multiples of min(ulp(q_j), s_q), within 2^25 of it)
+__host__ __device__ inline double code_query_resid2(float q, double sq, int32_t a) {
+  const double r = (double)q - sq * (double)a;
+  return r * r;
+}
+
+// the per-query constants from sum a, sum a^2 (exact), sum of code_query_resid2 (ss) and whether every q_j is finite
+__host__ __device__ inline CodeQuery code_query_finish(double sq, int32_t suma, double suma2, double ss, bool finite) {
+  CodeQuery c;
+  c.q2 = sq * sq * suma2;
+  c.sq2 = 2.0 * sq;
+  c.suma = suma;
+  // ss carries at most (2 ld) f64 roundings, far below the 2^-30 the two factors add
+  c.eq = finite ? sqrt(ss * (1.0 + 0x1p-30)) * (1.0 + 0x1p-30) : INFINITY;
+  if (!(c.eq <= 1.7976931348623157e308)) c.eq = INFINITY;
+  return c;
+}
+
+// The reference form of the preparation (the search does the same per lane and sums across the warp): a[0..ld) and the
+// constants for the query q[0..ld).
+__host__ __device__ inline CodeQuery code_query_prepare(const float* q, uint32_t ld, int32_t* a) {
+  float m = 0.f;
+  bool finite = true;
+  for (uint32_t j = 0; j < ld; ++j) {
+    finite = finite && code_finite(q[j]);
+    m = fmaxf(m, fabsf(q[j]));
+  }
+  const int32_t A = code_query_amax(ld);
+  const double sq = code_query_scale(finite ? m : 0.f, A);
+  int32_t suma = 0;
+  double suma2 = 0.0, ss = 0.0;
+  for (uint32_t j = 0; j < ld; ++j) {
+    a[j] = code_query_level(q[j], sq, A);
+    suma += a[j];
+    suma2 += (double)a[j] * (double)a[j];
+    ss += code_query_resid2(q[j], sq, a[j]);
+  }
+  return code_query_finish(sq, suma, suma2, ss, finite);
+}
+
+// The radius the integer test compares with: e_q + W, once per value of the beam's worst distance.
+__host__ __device__ inline double code_int_radius(const CodeQuery& cq, float worst) { return cq.eq + code_prune_radius(worst); }
+
+// Whether the row with header hdr = {lo, scale, err, X2} and S = sum a_j c_j can be dropped; WE = code_int_radius.
+__host__ __device__ inline bool code_int_prunes(const CodeQuery& cq, int32_t S, const float* hdr, double WE) {
+  const double x = (double)hdr[0] * (double)cq.suma, y = (double)hdr[1] * (double)S, X2 = (double)hdr[3];
+  const double dlo = (cq.q2 + X2) - cq.sq2 * (x + y) - 0x1p-45 * (cq.q2 + X2 + cq.sq2 * (fabs(x) + fabs(y)));
+  const double r = (double)hdr[2] + WE;
+  return dlo <= 1.7976931348623157e308 && dlo >= r * r;
 }
 
 // Fills the code rows of vectors ids[i] (ids == nullptr: first + i) for i < count.  One thread per row: this runs

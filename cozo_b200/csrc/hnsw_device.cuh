@@ -254,14 +254,82 @@ __device__ __forceinline__ void visit_clear(WarpCtx& w, int lane) {
   __syncwarp();
 }
 
-// f32 L2 distances from the query to two dequantised code rows in shared memory, each in dist_smem's lane-strided order
-// (the order codes_bound_emu.cpp checks the bound in).  The two FMA chains and shuffle trees are independent, so one
-// warp keeps twice the work in flight.
+// The query in the fixed point of the integer bound (hnsw_codes.cuh, CodeQuery), in the layout of the code words: the
+// lane that reads code word idx = lane + 32 i (elements 4 idx .. 4 idx + 3) owns a[32 i + lane] = {the int16 pair of
+// elements 4 idx, 4 idx + 1; that of 4 idx + 2, 4 idx + 3} (low half = lower element).  a lives in the warp's shared
+// memory (ceil(ld / 128) * 256 bytes; in registers the pruned kernel spills), and each lane reads only what it wrote.
+struct alignas(8) QueryPair {
+  uint32_t lo, hi;
+};
+struct QueryCodes {
+  QueryPair* a;
+  CodeQuery c;
+};
+
+// code_query_prepare of hnsw_codes.cuh, across the warp: the same per-element functions, the sums in lane order
 template <int NV>
-__device__ __forceinline__ void code_dist2(const float4 (&q)[NV], const uint8_t* r0, const uint8_t* r1, int lane,
-                                           int nvec4, float& d0, float& d1) {
-  const float lo0 = reinterpret_cast<const float*>(r0)[0], scale0 = reinterpret_cast<const float*>(r0)[1];
-  const float lo1 = reinterpret_cast<const float*>(r1)[0], scale1 = reinterpret_cast<const float*>(r1)[1];
+__device__ __forceinline__ void load_query_codes(const float4 (&q)[NV], uint32_t ld, int lane, QueryCodes& qc) {
+  float m = 0.f;
+  bool finite = true;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const float v[4] = {q[i].x, q[i].y, q[i].z, q[i].w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      finite = finite && code_finite(v[k]);
+      m = fmaxf(m, fabsf(v[k]));
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  finite = __ballot_sync(0xffffffffu, !finite) == 0u;
+  const int32_t A = code_query_amax(ld);
+  const double sq = code_query_scale(finite ? m : 0.f, A);
+  int32_t suma = 0;
+  double suma2 = 0.0, ss = 0.0;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {  // elements past ld are zero (load_query): a = 0, no residual
+    const float v[4] = {q[i].x, q[i].y, q[i].z, q[i].w};
+    int32_t a[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      a[k] = code_query_level(v[k], sq, A);
+      suma += a[k];
+      suma2 += (double)a[k] * (double)a[k];
+      ss += code_query_resid2(v[k], sq, a[k]);
+    }
+    if (32 * i < (int)ld / 4)
+      qc.a[32 * i + lane] = QueryPair{((uint32_t)a[0] & 0xFFFFu) | ((uint32_t)a[1] << 16),
+                                      ((uint32_t)a[2] & 0xFFFFu) | ((uint32_t)a[3] << 16)};
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    suma += __shfl_xor_sync(0xffffffffu, suma, o);
+    suma2 += __shfl_xor_sync(0xffffffffu, suma2, o);
+    ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  }
+  qc.c = code_query_finish(sq, suma, suma2, ss, finite);
+}
+
+// acc + the exact integer dot product of the four int16 query levels in (alo, ahi) with the four uint8 codes of c
+__device__ __forceinline__ int32_t code_idot4(uint32_t alo, uint32_t ahi, uint32_t c, int32_t acc) {
+#if defined(__CUDA_ARCH__)
+  // dp2a: two 16x8-bit products per instruction, int16 pairs against the low (.lo) or high (.hi) two code bytes
+  asm("dp2a.lo.s32.u32 %0, %1, %2, %0;" : "+r"(acc) : "r"(alo), "r"(c));
+  asm("dp2a.hi.s32.u32 %0, %1, %2, %0;" : "+r"(acc) : "r"(ahi), "r"(c));
+#else
+  acc += (int32_t)(int16_t)(alo & 0xFFFFu) * (int32_t)(c & 0xFFu) + (int32_t)(int16_t)(alo >> 16) * (int32_t)((c >> 8) & 0xFFu) +
+         (int32_t)(int16_t)(ahi & 0xFFFFu) * (int32_t)((c >> 16) & 0xFFu) + (int32_t)(int16_t)(ahi >> 16) * (int32_t)(c >> 24);
+#endif
+  return acc;
+}
+
+// S = sum_j a_j c_j (CodeQuery) for two code rows in shared memory, exact in int32 (so any summation order gives the same
+// S).  Each row's words alternate between two dp2a chains, and the warp sum is one redux.sync per row: the scoring is
+// bound by this chain's latency, not by issue.
+template <int NV>
+__device__ __forceinline__ void code_idot2(const QueryCodes& qc, const uint8_t* r0, const uint8_t* r1, int lane,
+                                           int nvec4, int32_t& s0, int32_t& s1) {
   const uint32_t* c0 = reinterpret_cast<const uint32_t*>(r0 + CODE_HDR);
   const uint32_t* c1 = reinterpret_cast<const uint32_t*>(r1 + CODE_HDR);
   // every shared-memory load first, so their latencies overlap (above NV = 8 that needs more registers than the
@@ -276,44 +344,28 @@ __device__ __forceinline__ void code_dist2(const float4 (&q)[NV], const uint8_t*
       w1[i] = idx < nvec4 ? c1[idx] : 0u;
     }
   }
-  float a0 = 0.f, a1 = 0.f, b = 0.f;
+  int32_t a0[2] = {0, 0}, a1[2] = {0, 0};
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     int idx = lane + 32 * i;
     if (idx < nvec4) {
-      const uint32_t u0 = HOIST ? w0[i] : c0[idx], u1 = HOIST ? w1[i] : c1[idx];
-      float4 v0, v1;
-#if defined(__CUDA_ARCH__)
-      // byte k of u as an exact float: 2^23 + u_k with the exponent bits spliced in by PRMT, minus 2^23 (no I2F)
-      v0.x = fmaf(__uint_as_float(__byte_perm(u0, 0x4B000000u, 0x7650)) - 8388608.f, scale0, lo0);
-      v0.y = fmaf(__uint_as_float(__byte_perm(u0, 0x4B000000u, 0x7651)) - 8388608.f, scale0, lo0);
-      v0.z = fmaf(__uint_as_float(__byte_perm(u0, 0x4B000000u, 0x7652)) - 8388608.f, scale0, lo0);
-      v0.w = fmaf(__uint_as_float(__byte_perm(u0, 0x4B000000u, 0x7653)) - 8388608.f, scale0, lo0);
-      v1.x = fmaf(__uint_as_float(__byte_perm(u1, 0x4B000000u, 0x7650)) - 8388608.f, scale1, lo1);
-      v1.y = fmaf(__uint_as_float(__byte_perm(u1, 0x4B000000u, 0x7651)) - 8388608.f, scale1, lo1);
-      v1.z = fmaf(__uint_as_float(__byte_perm(u1, 0x4B000000u, 0x7652)) - 8388608.f, scale1, lo1);
-      v1.w = fmaf(__uint_as_float(__byte_perm(u1, 0x4B000000u, 0x7653)) - 8388608.f, scale1, lo1);
-#else
-      v0.x = code_value(u0 & 0xFFu, lo0, scale0);
-      v0.y = code_value((u0 >> 8) & 0xFFu, lo0, scale0);
-      v0.z = code_value((u0 >> 16) & 0xFFu, lo0, scale0);
-      v0.w = code_value(u0 >> 24, lo0, scale0);
-      v1.x = code_value(u1 & 0xFFu, lo1, scale1);
-      v1.y = code_value((u1 >> 8) & 0xFFu, lo1, scale1);
-      v1.z = code_value((u1 >> 16) & 0xFFu, lo1, scale1);
-      v1.w = code_value(u1 >> 24, lo1, scale1);
-#endif
-      accum<COZO_GPU_L2>(q[i], v0, a0, b);
-      accum<COZO_GPU_L2>(q[i], v1, a1, b);
+      const QueryPair qa = qc.a[idx];
+      a0[i & 1] = code_idot4(qa.lo, qa.hi, HOIST ? w0[i] : c0[idx], a0[i & 1]);
+      a1[i & 1] = code_idot4(qa.lo, qa.hi, HOIST ? w1[i] : c1[idx], a1[i & 1]);
     }
   }
-#pragma unroll
+#if defined(__CUDA_ARCH__)
+  s0 = __reduce_add_sync(0xffffffffu, a0[0] + a0[1]);
+  s1 = __reduce_add_sync(0xffffffffu, a1[0] + a1[1]);
+#else
+  int32_t t0 = a0[0] + a0[1], t1 = a1[0] + a1[1];
   for (int o = 16; o > 0; o >>= 1) {
-    a0 += __shfl_xor_sync(0xffffffffu, a0, o);
-    a1 += __shfl_xor_sync(0xffffffffu, a1, o);
+    t0 += __shfl_xor_sync(0xffffffffu, t0, o);
+    t1 += __shfl_xor_sync(0xffffffffu, t1, o);
   }
-  d0 = a0;
-  d1 = a1;
+  s0 = t0;
+  s1 = t1;
+#endif
 }
 
 // One 32-id adjacency chunk of a pruned hop (L2, codes present, beam full), as one stream per warp.  `id` is this lane's
@@ -321,7 +373,8 @@ __device__ __forceinline__ void code_dist2(const float4 (&q)[NV], const uint8_t*
 //   * The code rows of the first w.cns valid ids are issued before the visited test, so their fetch overlaps the
 //     atomicOr round trip.  Those that turn out to be visited are waited for and discarded (not scored, not counted);
 //     later ids are fetched only if they are unvisited.  Stream position p holds w.pend[p], bit 31 set = discard.
-//   * Each code row is bounded from below (hnsw_codes.cuh) against the beam's worst distance AT THAT MOMENT.  With a
+//   * Each code row is bounded from below (hnsw_codes.cuh, code_int_prunes: from the exact integer product of the code
+//     row with the fixed-point query qc) against the beam's worst distance AT THAT MOMENT.  With a
 //     full beam fd[len-1] only decreases, and a neighbour's admission test `d < fd[len-1]` comes after every earlier
 //     survivor's admission, so the value tested here is at least the one its admission would face: a dropped
 //     neighbour could not have been admitted.
@@ -330,8 +383,8 @@ __device__ __forceinline__ void code_dist2(const float4 (&q)[NV], const uint8_t*
 //     Admissions therefore happen in neighbour order with the live bound, exactly as without pruning: ids, distances
 //     and the traversal counters are unchanged; only the number of f32 rows fetched can go down.
 template <int NV>
-__device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const float4 (&q)[NV], uint32_t ef,
-                                            uint32_t id, uint32_t validmask, int lane) {
+__device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const float4 (&q)[NV], const QueryCodes& qc,
+                                            uint32_t ef, uint32_t id, uint32_t validmask, int lane) {
   const int nvec4 = g.ld >> 2;
   const uint32_t crow = g.code_ld, row_bytes = g.ld * 4;
   const uint32_t lt = (1u << lane) - 1;
@@ -357,7 +410,7 @@ __device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const 
   HOP_ADD(w, HC_VISIT, t0);
 
   uint32_t fq = 0, fin = 0;  // bits by stream position: survivors whose f32 row is queued / in flight (in order)
-  double W = code_prune_radius(w.fd[ef - 1]);
+  double WE = code_int_radius(qc.c, w.fd[ef - 1]);
   // f32 ring: slot w.head holds the oldest row in flight, popc(fin) rows are in flight
   auto f32_issue = [&]() {
     while (fq && __popc(fin) < w.ns) {
@@ -388,12 +441,12 @@ __device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const 
     __syncwarp();
     if (d < w.fd[ef - 1]) {  // hnsw.rs:575-581 (the beam stays full)
       sorted_insert(w, ef, d, nid, lane);
-      W = code_prune_radius(w.fd[ef - 1]);
+      WE = code_int_radius(qc.c, w.fd[ef - 1]);
     }
     HOP_ADD(w, HC_FSCORE, t2);
   };
 
-  // code rows two at a time (code_dist2); position `issued` is the next one to fetch, into slot chead + issued - c
+  // code rows two at a time (code_idot2); position `issued` is the next one to fetch, into slot chead + issued - c
   uint32_t issued = spec;
   for (uint32_t c = 0; c < len;) {
     const uint32_t upto = min(len, c + w.cns);
@@ -421,17 +474,17 @@ __device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const 
     HOP_T(t4);
     const uint8_t* r0 = w.cring + (size_t)w.chead * crow;
     const uint8_t* r1 = two ? w.cring + (size_t)s1 * crow : r0;
-    float dt0, dt1;
-    code_dist2<NV>(q, r0, r1, lane, nvec4, dt0, dt1);
-    const float err0 = reinterpret_cast<const float*>(r0)[2], err1 = reinterpret_cast<const float*>(r1)[2];
+    int32_t S0, S1;
+    code_idot2<NV>(qc, r0, r1, lane, nvec4, S0, S1);
+    const float4 h0 = *reinterpret_cast<const float4*>(r0), h1 = *reinterpret_cast<const float4*>(r1);
     const uint32_t p0 = w.pend[c], p1 = two ? w.pend[c + 1] : EXPANDED;
     __syncwarp();  // every lane is done with the two slots before lane 0 refills them
     if (!(p0 & EXPANDED)) {
-      if (code_prunes(dt0, err0, W)) w.pruned++;
+      if (code_int_prunes(qc.c, S0, &h0.x, WE)) w.pruned++;
       else fq |= 1u << c;
     }
     if (!(p1 & EXPANDED)) {
-      if (code_prunes(dt1, err1, W)) w.pruned++;
+      if (code_int_prunes(qc.c, S1, &h1.x, WE)) w.pruned++;
       else fq |= 1u << (c + 1);
     }
     const uint32_t step = two ? 2 : 1;
@@ -456,9 +509,11 @@ __device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const 
 // `level` 0 is the bottom layer.  On entry the sorted array holds found_nn.
 // PRUNE (L2 with the bulk ring): when g.codes is set, the chunks of a hop that find the beam full run prune_chunk, which
 // fetches f32 rows only for the neighbours whose code row cannot rule out admission.
+// qc: the query's fixed-point form (load_query_codes), read only by prune_chunk.
 template <int NV, int METRIC, bool BULK, bool PRUNE = false>
 __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const float4 (&q)[NV], float qnorm,
-                                             uint32_t ef, uint32_t level, int lane) {
+                                             uint32_t ef, uint32_t level, int lane,
+                                             const QueryCodes* qc = nullptr) {
   const int nvec4 = g.ld >> 2;
   const uint32_t row_bytes = g.ld * 4;
   // visited <- keys(found); candidates <- found (hnsw.rs:554-557)
@@ -517,7 +572,7 @@ __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const
       if (!validmask) break;
       w.nbr_reads += __popc(validmask);
       if (PRUNE && g.codes && w.len == ef) {
-        prune_chunk<NV>(g, w, q, ef, id, validmask, lane);
+        prune_chunk<NV>(g, w, q, *qc, ef, id, validmask, lane);
         __syncwarp();
         continue;
       }
