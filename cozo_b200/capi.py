@@ -23,7 +23,7 @@ E_INVAL, E_CUDA, E_NODEV, E_NOMEM, E_KILLED, E_UNSUP = -1, -2, -3, -4, -5, -6
 EXPORTS = [
     "cozo_gpu_init", "cozo_gpu_shutdown", "cozo_gpu_last_error", "cozo_gpu_device_count", "cozo_gpu_set_option",
     "cozo_gpu_get_option", "cozo_gpu_hnsw_stage", "cozo_gpu_hnsw_free", "cozo_gpu_hnsw_search",
-    "cozo_gpu_hnsw_search_dev", "cozo_gpu_hnsw_search_scatter_dev", "cozo_gpu_hnsw_build", "cozo_gpu_hnsw_insert", "cozo_gpu_hnsw_remove", "cozo_gpu_hnsw_update", "cozo_gpu_hnsw_info", "cozo_gpu_hnsw_level_size",
+    "cozo_gpu_hnsw_search_dev", "cozo_gpu_hnsw_search_scatter_dev", "cozo_gpu_hnsw_build", "cozo_gpu_hnsw_insert", "cozo_gpu_hnsw_insert_at", "cozo_gpu_hnsw_remove", "cozo_gpu_hnsw_update", "cozo_gpu_hnsw_info", "cozo_gpu_hnsw_level_size",
     "cozo_gpu_hnsw_export_level", "cozo_gpu_hnsw_export_level_dist", "cozo_gpu_hnsw_export_live", "cozo_gpu_hnsw_vectors_dev", "cozo_gpu_topk_merge_dev", "cozo_gpu_graph_stage",
     "cozo_gpu_graph_free", "cozo_gpu_graph_export", "cozo_gpu_pagerank", "cozo_gpu_sssp_multi", "cozo_gpu_closeness",
     "cozo_gpu_betweenness", "cozo_gpu_clustering", "cozo_gpu_sssp_paths",
@@ -88,6 +88,7 @@ def load():
     L.cozo_gpu_hnsw_search_scatter_dev.argtypes = [vp, vp, u32, u32, u32, f64, u32, vp, vp, u32, vp, vp]
     L.cozo_gpu_hnsw_build.argtypes = [C.POINTER(vp), C.POINTER(HnswBuildDesc)]
     L.cozo_gpu_hnsw_insert.argtypes = [vp, vp, u32, C.c_int32, u32, C.c_int32, vp]
+    L.cozo_gpu_hnsw_insert_at.argtypes = [vp, vp, vp, u32, C.c_int32, u32, C.c_int32, vp]
     L.cozo_gpu_hnsw_remove.argtypes = [vp, vp, u32]
     L.cozo_gpu_hnsw_update.argtypes = [vp, vp, vp, u32, u32, C.c_int32]
     L.cozo_gpu_hnsw_info.argtypes = [vp, vp, vp, vp, vp]
@@ -243,6 +244,17 @@ class HnswIndex:
         _check(load().cozo_gpu_hnsw_insert(self._h, _p(vectors), vectors.shape[0], 0, ef_construction,
                                            keep_pruned_connections, C.byref(first)))
         return first.value
+
+    def insert_at(self, positions, vectors: np.ndarray, ef_construction: int = 0,
+                  keep_pruned_connections: int = -1) -> np.ndarray:
+        """hnsw_put of new rows at any key position: positions[i] = ids whose key sorts before row i (non-decreasing).
+        Existing ids move up to keep dense ids in key order; returns the new rows' ids (positions[i] + i)."""
+        positions = np.ascontiguousarray(positions, np.uint32)
+        vectors = np.ascontiguousarray(vectors, np.float32).reshape(positions.size, self.dim)
+        out = np.zeros(positions.size, np.uint32)
+        _check(load().cozo_gpu_hnsw_insert_at(self._h, _p(positions), _p(vectors), positions.size, 0, ef_construction,
+                                              keep_pruned_connections, _p(out)))
+        return out
 
     def update(self, ids, vectors, ef_construction: int = 0, keep_pruned_connections: int = -1):
         """hnsw_put of changed vectors under existing ids (remove + insert again, hnsw.rs:175-182)"""

@@ -239,11 +239,17 @@ int hnsw_ensure_build_state(cozo_gpu_hnsw* h) {
   return 0;
 }
 
-// The batched insertion loop for nodes [begin, end) whose vectors, levels and upper_off are in place.
-int hnsw_insert_range(cozo_gpu_hnsw* h, uint32_t begin, uint32_t end, uint32_t max_batch) {
+// f32 row stages per warp of the K1 search
+static uint32_t build_stages() { return std::min(32u, std::max(1u, (uint32_t)get_option("hnsw.stages", 4))); }
+
+// The batched insertion loop for the nodes `ids` (ascending) whose vectors, levels and upper_off are in place, linked in
+// list order.  min_entry: after each batch the entry is the smallest id on the top layer (a node inserted at a key
+// before the entry's, on the entry's layer, takes over, hnsw.rs:184-199); otherwise only a higher layer re-points it.
+static int hnsw_insert_ids(cozo_gpu_hnsw* h, const std::vector<uint32_t>& ids, uint32_t max_batch, bool min_entry) {
   const DeviceInfo& di = device_info();
   HnswDev& g = h->dev;
-  if (begin >= end) return 0;
+  const uint32_t total = (uint32_t)ids.size();
+  if (total == 0) return 0;
   K1Fn k1, k2;
   K4Fn k4;
   KdFn kd;
@@ -258,8 +264,7 @@ int hnsw_insert_range(cozo_gpu_hnsw* h, uint32_t begin, uint32_t end, uint32_t m
   if (extend) max_batch = 1;
   uint32_t wpc = (uint32_t)get_option("hnsw.warps_per_cta", 4);
   wpc = std::min(4u, std::max(1u, wpc));
-  uint32_t ns = (uint32_t)get_option("hnsw.stages", 4);
-  ns = std::min(32u, std::max(1u, ns));
+  const uint32_t ns = build_stages();
   SmemLayout lay = make_layout(ef_c, ns, g.ld);
   size_t smem1 = (size_t)lay.warp_bytes * wpc;
   while (smem1 > di.smem_optin && wpc > 1) {
@@ -309,9 +314,9 @@ int hnsw_insert_range(cozo_gpu_hnsw* h, uint32_t begin, uint32_t end, uint32_t m
     rc = hnsw_ws_reserve(ws, slots * nwords, slots * logcap, st);
     if (rc) return rc;
   }
-  max_batch = std::min<uint32_t>(max_batch, end - begin);
+  max_batch = std::min<uint32_t>(max_batch, total);
   uint32_t max_lvl = 0;
-  for (uint32_t i = begin; i < end; ++i) max_lvl = std::max<uint32_t>(max_lvl, h->node_level[i]);
+  for (uint32_t id : ids) max_lvl = std::max<uint32_t>(max_lvl, h->node_level[id]);
   const uint32_t Tcap = (uint32_t)std::min<uint64_t>((uint64_t)max_batch * (max_lvl + 1), (uint64_t)max_batch + h->up_rows + 16);
   const uint64_t req_cap = std::max<uint64_t>((uint64_t)Tcap * mcap, 1);
   H_CUDA(cudaMalloc(&sc.coff, ((size_t)max_batch + 1) * 4));
@@ -352,24 +357,24 @@ int hnsw_insert_range(cozo_gpu_hnsw* h, uint32_t begin, uint32_t end, uint32_t m
     H_CUDA(cudaMemcpy(sc.perm, iota.data(), req_cap * 4, cudaMemcpyHostToDevice));
   }
 
-  uint32_t inserted = begin;
+  uint32_t inserted = 0;  // position in `ids`
   if (g.entry == NONE) {  // first vector: fresh self-loops only (hnsw.rs:360-373)
-    g.entry = begin;
-    g.top_level = h->node_level[begin];
-    inserted = begin + 1;
+    g.entry = ids[0];
+    g.top_level = h->node_level[ids[0]];
+    inserted = 1;
     h->n_live += 1;
   }
   std::vector<uint32_t> coff, lnode, llevel;
-  while (inserted < end) {
+  while (inserted < total) {
     // a batch never exceeds 1/16 of what is already linked, so that batch members (which do not see
     // each other) stay a small fraction of every neighbourhood
-    uint32_t bs = std::min<uint32_t>(std::min<uint32_t>(max_batch, std::max<uint32_t>(1u, h->n_live / 16)), end - inserted);
+    uint32_t bs = std::min<uint32_t>(std::min<uint32_t>(max_batch, std::max<uint32_t>(1u, h->n_live / 16)), total - inserted);
     const uint32_t top = g.top_level;
     coff.assign(bs + 1, 0);
     lnode.clear();
     llevel.clear();
     for (uint32_t i = 0; i < bs; ++i) {
-      uint32_t id = inserted + i;
+      uint32_t id = ids[inserted + i];
       uint32_t nl = std::min<uint32_t>(h->node_level[id], top) + 1;
       coff[i] = (uint32_t)lnode.size();
       for (uint32_t L = 0; L < nl; ++L) {
@@ -385,7 +390,7 @@ int hnsw_insert_range(cozo_gpu_hnsw* h, uint32_t begin, uint32_t end, uint32_t m
     H_CUDA(cudaMemcpyAsync(sc.list_level, llevel.data(), (size_t)T * 4, cudaMemcpyHostToDevice, st));
     H_CUDA(cudaMemsetAsync(sc.counters, 0, 64, st));
     BatchParams p{};
-    p.begin = inserted;
+    p.begin = ids[inserted];
     p.count = bs;
     p.top = top;
     p.ef_c = ef_c;
@@ -438,9 +443,11 @@ int hnsw_insert_range(cozo_gpu_hnsw* h, uint32_t begin, uint32_t end, uint32_t m
     // a node above the current top becomes the entry point (hnsw.rs:206-218);
     // the entry is the smallest id on the top layer (hnsw.rs:184-199)
     for (uint32_t i = 0; i < bs; ++i) {
-      uint32_t id = inserted + i;
+      uint32_t id = ids[inserted + i];
       if (h->node_level[id] > g.top_level) {
         g.top_level = h->node_level[id];
+        g.entry = id;
+      } else if (min_entry && h->node_level[id] == g.top_level && id < g.entry) {
         g.entry = id;
       }
     }
@@ -452,24 +459,42 @@ int hnsw_insert_range(cozo_gpu_hnsw* h, uint32_t begin, uint32_t end, uint32_t m
   return 0;
 }
 
+// hnsw_insert_ids for the id range [begin, end)
+int hnsw_insert_range(cozo_gpu_hnsw* h, uint32_t begin, uint32_t end, uint32_t max_batch) {
+  std::vector<uint32_t> ids;
+  for (uint32_t id = begin; id < end; ++id) ids.push_back(id);
+  return hnsw_insert_ids(h, ids, max_batch, false);
+}
+
+// levels of `count` new rows, drawn in row order from the handle's seeded level law (hnsw.rs:46-52),
+// level_multiplier = 1/ln(m) (relation.rs:1147)
+static std::vector<uint8_t> draw_levels(cozo_gpu_hnsw* h, uint32_t count) {
+  SplitMix64 rng{h->rng_state};
+  const double mult = 1.0 / std::log((double)h->m_max);
+  std::vector<uint8_t> lv(count);
+  for (uint32_t i = 0; i < count; ++i) {
+    double u = rng.uniform();
+    double r = -std::log(u) * mult;
+    if (!(r < 15.0)) r = 15.0;
+    lv[i] = (uint8_t)std::floor(r);
+  }
+  h->rng_state = rng.s;
+  return lv;
+}
+
 // append `count` vectors as ids [n, n+count): levels from the handle's RNG, rows and capacity
 static int append_nodes(cozo_gpu_hnsw* h, const float* vectors, int on_device, uint32_t count) {
   HnswDev& g = h->dev;
   const uint32_t n0 = g.n, n1 = n0 + count;
   if ((uint64_t)n0 + count >= 0x7FFFFFFFull) return set_error(COZO_GPU_EUNSUP, "too many vectors");
-  // level law (hnsw.rs:46-52), level_multiplier = 1/ln(m) (relation.rs:1147)
-  SplitMix64 rng{h->rng_state};
-  const double mult = 1.0 / std::log((double)h->m_max);
+  const std::vector<uint8_t> lvs = draw_levels(h, count);
   h->node_level.resize(n1, 0);
   h->live.resize(n1, 1);
   std::vector<uint32_t> upper_off(count, NONE);
   std::vector<uint32_t> owners;
   uint64_t up = h->up_rows;
   for (uint32_t i = 0; i < count; ++i) {
-    double u = rng.uniform();
-    double r = -std::log(u) * mult;
-    if (!(r < 15.0)) r = 15.0;
-    uint8_t lv = (uint8_t)std::floor(r);
+    const uint8_t lv = lvs[i];
     h->node_level[n0 + i] = lv;
     if (lv) {
       upper_off[i] = (uint32_t)up;
@@ -477,7 +502,6 @@ static int append_nodes(cozo_gpu_hnsw* h, const float* vectors, int on_device, u
       for (uint32_t L = 0; L < lv; ++L) owners.push_back(n0 + i);
     }
   }
-  h->rng_state = rng.s;
   int rc = hnsw_reserve(h, n1, up);
   if (rc) return rc;
   if (vectors)  // nullptr: the (borrowed) rows are already in place
@@ -547,14 +571,8 @@ extern "C" int cozo_gpu_hnsw_build(cozo_gpu_hnsw_t** out, const CozoGpuHnswBuild
   return 0;
 }
 
-// hnsw_put for rows that sort after every indexed key (query/stored.rs:332 -> hnsw.rs:679-727).
-extern "C" int cozo_gpu_hnsw_insert(cozo_gpu_hnsw_t* h, const float* vectors, uint32_t count, int32_t vectors_on_device,
-                                    uint32_t ef_construction, int32_t keep_pruned_connections, uint32_t* first_id) {
-  if (!h || (count && !vectors)) return set_error(COZO_GPU_EINVAL, "null argument");
-  int rc = ensure_init();
-  if (rc) return rc;
-  if (first_id) *first_id = h->dev.n;
-  if (count == 0) return 0;
+// The settings and build state an insertion needs (shared by insert and insert_at).
+static int prepare_insert(cozo_gpu_hnsw* h, uint32_t ef_construction, int32_t keep_pruned_connections) {
   // A handle staged from the canary row alone (n = 0) grows from empty arrays: hnsw_ensure_build_state gives it
   // capacities equal to its live rows (0), so every row the first insert creates is initialised by grow().
   if (h->m_max < 2 || h->m_max > 64) return set_error(COZO_GPU_EUNSUP, "m_neighbours must be in [2,64] for the device builder");
@@ -563,12 +581,194 @@ extern "C" int cozo_gpu_hnsw_insert(cozo_gpu_hnsw_t* h, const float* vectors, ui
   if (keep_pruned_connections >= 0) h->keep_pruned = keep_pruned_connections;
   // a staged handle learns the manifest's extend_candidates through the option (a built handle keeps its own)
   if (get_option("hnsw.extend_candidates", -1) >= 0) h->extend_candidates = get_option("hnsw.extend_candidates", 0) != 0;
-  rc = hnsw_ensure_build_state(h);
+  return hnsw_ensure_build_state(h);
+}
+
+// hnsw_put for rows that sort after every indexed key (query/stored.rs:332 -> hnsw.rs:679-727).
+extern "C" int cozo_gpu_hnsw_insert(cozo_gpu_hnsw_t* h, const float* vectors, uint32_t count, int32_t vectors_on_device,
+                                    uint32_t ef_construction, int32_t keep_pruned_connections, uint32_t* first_id) {
+  if (!h || (count && !vectors)) return set_error(COZO_GPU_EINVAL, "null argument");
+  int rc = ensure_init();
+  if (rc) return rc;
+  if (first_id) *first_id = h->dev.n;
+  if (count == 0) return 0;
+  rc = prepare_insert(h, ef_construction, keep_pruned_connections);
   if (rc) return rc;
   const uint32_t n0 = h->dev.n;
   rc = append_nodes(h, vectors, vectors_on_device, count);
   if (rc) return rc;
   return hnsw_insert_range(h, n0, n0 + count, 0);
+}
+
+// Moves rows [first, n) of one per-node array (row_bytes each) to their relabelled rows, `chunk` rows at a time from the
+// tail through `stage`.  Destinations are never below their sources, so a chunk only overwrites rows already moved, and
+// no second copy of the array is needed.  On the legacy default stream.
+static int shift_rows(void* base, size_t row_bytes, uint32_t first, uint32_t n, uint8_t* stage, uint64_t chunk,
+                      const uint32_t* d_pos, uint32_t npos) {
+  uint8_t* p = static_cast<uint8_t*>(base);
+  for (uint32_t hi = n; hi > first;) {
+    const uint32_t lo = hi - (uint32_t)std::min<uint64_t>(chunk, hi - first);
+    const uint32_t rows = hi - lo;
+    H_CUDA(cudaMemcpyAsync(stage, p + (size_t)lo * row_bytes, (size_t)rows * row_bytes, cudaMemcpyDeviceToDevice, 0));
+    if (row_bytes % 16 == 0) {
+      const uint32_t e = (uint32_t)(row_bytes / 16);
+      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
+      shift_rows_kernel<uint4><<<(uint32_t)((threads + 255) / 256), 256>>>(
+          reinterpret_cast<const uint4*>(stage), reinterpret_cast<uint4*>(p), e, lo, rows, d_pos, npos);
+    } else if (row_bytes % 4 == 0) {
+      const uint32_t e = (uint32_t)(row_bytes / 4);
+      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
+      shift_rows_kernel<uint32_t><<<(uint32_t)((threads + 255) / 256), 256>>>(
+          reinterpret_cast<const uint32_t*>(stage), reinterpret_cast<uint32_t*>(p), e, lo, rows, d_pos, npos);
+    } else {
+      const uint32_t e = (uint32_t)row_bytes;
+      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
+      shift_rows_kernel<uint8_t><<<(uint32_t)((threads + 255) / 256), 256>>>(stage, p, e, lo, rows, d_pos, npos);
+    }
+    H_CUDA(cudaGetLastError());
+    hi = lo;
+  }
+  return 0;
+}
+
+static int relabel_ids(uint32_t* ids, size_t count, const uint32_t* d_pos, uint32_t npos) {
+  if (!count) return 0;
+  relabel_ids_kernel<<<(uint32_t)((count + 255) / 256), 256>>>(ids, count, d_pos, npos);
+  H_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// hnsw_put of new rows at any key position (query/stored.rs:332 -> hnsw.rs:679-727).  Existing ids move up to open a
+// gap before every new row, so that dense ids stay in compound-key order; then the new ids are linked in one batched run.
+extern "C" int cozo_gpu_hnsw_insert_at(cozo_gpu_hnsw_t* h, const uint32_t* positions, const float* vectors, uint32_t count,
+                                       int32_t vectors_on_device, uint32_t ef_construction,
+                                       int32_t keep_pruned_connections, uint32_t* out_ids) {
+  if (!h || (count && (!positions || !vectors))) return set_error(COZO_GPU_EINVAL, "null argument");
+  int rc = ensure_init();
+  if (rc) return rc;
+  if (count == 0) return 0;
+  HnswDev& g = h->dev;
+  const uint32_t n0 = g.n;
+  for (uint32_t i = 0; i < count; ++i)
+    if (positions[i] > n0 || (i && positions[i] < positions[i - 1]))
+      return set_error(COZO_GPU_EINVAL, "positions must be non-decreasing and at most n = %u (row %u)", n0, i);
+  if ((uint64_t)n0 + count >= 0x7FFFFFFFull) return set_error(COZO_GPU_EUNSUP, "too many vectors");
+  // an asynchronous search_dev may still be reading the rows about to move (and ids up to its n)
+  H_CUDA(cudaDeviceSynchronize());
+  if (positions[0] == n0) {  // every row after every indexed key: an append
+    uint32_t first = 0;
+    rc = cozo_gpu_hnsw_insert(h, vectors, count, vectors_on_device, ef_construction, keep_pruned_connections, &first);
+    if (!rc && out_ids)
+      for (uint32_t i = 0; i < count; ++i) out_ids[i] = first + i;
+    return rc;
+  }
+  rc = prepare_insert(h, ef_construction, keep_pruned_connections);
+  if (rc) return rc;
+  // the builder needs at least one warp's shared memory: refuse before any row moves
+  if (make_layout(h->ef_construction, build_stages(), g.ld).warp_bytes > device_info().smem_optin)
+    return set_error(COZO_GPU_EUNSUP, "ef_construction=%u does not fit shared memory", h->ef_construction);
+
+  // scratch first, so that running out of memory leaves the index as it was
+  struct Scratch {
+    uint32_t *pos = nullptr, *ids = nullptr, *up_off = nullptr;
+    uint8_t *levels = nullptr, *stage = nullptr;
+    float* vec = nullptr;
+    ~Scratch() {
+      void* ptrs[] = {pos, ids, up_off, levels, stage, vec};
+      for (void* p : ptrs)
+        if (p) cudaFree(p);
+    }
+  } sc;
+  H_CUDA(cudaMalloc(&sc.pos, (size_t)count * 4));
+  H_CUDA(cudaMalloc(&sc.ids, (size_t)count * 4));
+  H_CUDA(cudaMalloc(&sc.up_off, (size_t)count * 4));
+  H_CUDA(cudaMalloc(&sc.levels, count));
+  if (!vectors_on_device) H_CUDA(cudaMalloc(&sc.vec, (size_t)count * g.dim * 4));
+  // Per-node arrays and their row sizes (code rows only where the index has them).  Each array moves through the
+  // staging buffer in chunks of kStageBytes / row_bytes rows, or of `hnsw.shift_chunk_rows` rows when that is set.
+  const size_t kStageBytes = (size_t)64 << 20;
+  const size_t vec_row = (size_t)g.ld * 4, adj_row = (size_t)g.s0 * 4;
+  const size_t row_bytes[] = {vec_row, g.code_ld, adj_row, adj_row, 4, 4, 1, 1};
+  const int64_t chunk_opt = get_option("hnsw.shift_chunk_rows", 0);
+  const uint64_t moving = n0 - positions[0];
+  auto chunk_rows = [&](size_t rb) {
+    const uint64_t c = chunk_opt > 0 ? (uint64_t)chunk_opt : std::max<uint64_t>(1, kStageBytes / rb);
+    return std::max<uint64_t>(1, std::min(c, moving));
+  };
+  size_t stage_bytes = 1;
+  for (size_t rb : row_bytes) stage_bytes = std::max(stage_bytes, (size_t)chunk_rows(rb) * rb);
+  H_CUDA(cudaMalloc(&sc.stage, stage_bytes));
+
+  if (!h->vec_owned) {  // never write into a borrowed buffer
+    rc = hnsw_reserve(h, h->borrowed_rows + 1, h->up_rows);
+    if (rc) return rc;
+  }
+  const uint32_t n1 = n0 + count;
+  const std::vector<uint8_t> lvs = draw_levels(h, count);
+  std::vector<uint32_t> new_ids(count), up_off(count, NONE), owners;
+  uint64_t up = h->up_rows;
+  for (uint32_t i = 0; i < count; ++i) {
+    new_ids[i] = positions[i] + i;
+    if (lvs[i]) {
+      up_off[i] = (uint32_t)up;
+      up += lvs[i];
+      for (uint32_t L = 0; L < lvs[i]; ++L) owners.push_back(new_ids[i]);
+    }
+  }
+  const uint64_t up0 = h->up_rows;
+  rc = hnsw_reserve(h, n1, up);
+  if (rc) return rc;
+  H_CUDA(cudaMemcpy(sc.pos, positions, (size_t)count * 4, cudaMemcpyHostToDevice));
+  H_CUDA(cudaMemcpy(sc.ids, new_ids.data(), (size_t)count * 4, cudaMemcpyHostToDevice));
+  H_CUDA(cudaMemcpy(sc.up_off, up_off.data(), (size_t)count * 4, cudaMemcpyHostToDevice));
+  H_CUDA(cudaMemcpy(sc.levels, lvs.data(), count, cudaMemcpyHostToDevice));
+  const float* d_new_vec = vectors;
+  if (!vectors_on_device) {
+    H_CUDA(cudaMemcpy(sc.vec, vectors, (size_t)count * g.dim * 4, cudaMemcpyHostToDevice));
+    d_new_vec = sc.vec;
+  }
+
+  // 1. every per-node array: old row j -> j + #{positions <= j}; rows below positions[0] stay
+  void* const bases[] = {h->d_vec, g.codes ? h->d_codes : nullptr, h->d_adj0, h->d_adj0_dist,
+                         h->d_deg0, h->d_upper_off, h->d_node_level, h->d_dead};
+  for (size_t a = 0; a < 8; ++a) {
+    if (!bases[a]) continue;
+    rc = shift_rows(bases[a], row_bytes[a], positions[0], n0, sc.stage, chunk_rows(row_bytes[a]), sc.pos, count);
+    if (rc) return rc;
+  }
+  // 2. the new rows
+  place_new_rows_kernel<<<(uint32_t)(((uint64_t)count * 32 + 255) / 256), 256>>>(
+      sc.ids, count, d_new_vec, g.dim, h->d_vec, g.ld, h->d_adj0, g.s0, h->d_deg0, sc.up_off, h->d_upper_off,
+      sc.levels, h->d_node_level, h->d_dead);
+  H_CUDA(cudaGetLastError());
+  hnsw_codes_fill(h, 0, count, sc.ids);
+  // 3. every stored id; adj_up rows stay where they are (upper_off holds row numbers)
+  rc = relabel_ids(h->d_adj0, (size_t)n1 * g.s0, sc.pos, count);
+  if (!rc) rc = relabel_ids(h->d_adj_up, (size_t)up0 * g.su, sc.pos, count);
+  if (!rc) rc = relabel_ids(h->d_up_owner, (size_t)up0, sc.pos, count);
+  if (rc) return rc;
+  if (!owners.empty())
+    H_CUDA(cudaMemcpyAsync(h->d_up_owner + up0, owners.data(), owners.size() * 4, cudaMemcpyHostToDevice, 0));
+  H_CUDA(cudaDeviceSynchronize());  // the builder runs on a workspace stream, which the legacy stream does not order
+
+  // host copies
+  std::vector<uint8_t> level(n1), live(n1, 1);
+  for (uint32_t j = 0, i = 0; j < n0; ++j) {
+    while (i < count && positions[i] <= j) ++i;
+    level[j + i] = h->node_level[j];
+    live[j + i] = h->live[j];
+  }
+  for (uint32_t i = 0; i < count; ++i) level[new_ids[i]] = lvs[i];
+  h->node_level.swap(level);
+  h->live.swap(live);
+  if (g.entry != NONE)
+    g.entry += (uint32_t)(std::upper_bound(positions, positions + count, g.entry) - positions);
+  h->up_rows = up;
+  g.n = n1;
+  rc = hnsw_insert_ids(h, new_ids, 0, true);
+  if (rc) return rc;
+  if (out_ids) std::copy(new_ids.begin(), new_ids.end(), out_ids);
+  return 0;
 }
 
 // hnsw_remove (hnsw.rs:728-868) for a batch of ids.

@@ -40,7 +40,8 @@ struct BuildDev {
 };
 
 struct BatchParams {
-  uint32_t begin, count;  // node ids [begin, begin+count)
+  uint32_t begin;         // id of the batch's first node; the kernels read ids from list_node
+  uint32_t count;         // nodes in the batch; node i is list_node[coff[i]]
   uint32_t top;           // top layer before the batch
   uint32_t ef_c;
   const uint32_t* coff;        // [count+1] first candidate list of node i
@@ -98,7 +99,8 @@ __device__ __forceinline__ void build_search_body(const HnswDev& g, const BuildD
     if (lane == 0) i = atomicAdd(p.counter, 1u);
     i = __shfl_sync(0xffffffffu, i, 0);
     if (i >= p.count) break;
-    const uint32_t id = p.begin + i;
+    const uint32_t l0 = p.coff[i];
+    const uint32_t id = p.list_node[l0];
     const uint32_t lq = b.node_level[id];
     float4 q[NV];
     float qnorm;
@@ -115,7 +117,6 @@ __device__ __forceinline__ void build_search_body(const HnswDev& g, const BuildD
     __syncwarp();
     for (uint32_t L = p.top; L > lq; --L) search_level<NV, METRIC, true>(g, w, q, qnorm, 1, L, lane);
     uint32_t L = lq < p.top ? lq : p.top;
-    const uint32_t l0 = p.coff[i];
     for (;; --L) {
       search_level<NV, METRIC, true>(g, w, q, qnorm, p.ef_c, L, lane);
       const size_t list = (size_t)(l0 + L) * p.ef_c;
@@ -546,6 +547,61 @@ __global__ void __launch_bounds__(128) remove_compact_kernel(uint32_t* adj, floa
 __global__ void mark_dead_kernel(const uint32_t* ids, uint32_t count, uint8_t* dead) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < count) dead[ids[i]] = 1;
+}
+
+// ---- insert at any key position (cozo_gpu_hnsw_insert_at) -------------------------------------------------------
+// pos: the ascending insert positions.  Old id j becomes j + #{i : pos[i] <= j}.
+__device__ __forceinline__ uint32_t relabel_id(const uint32_t* pos, uint32_t npos, uint32_t id) {
+  uint32_t lo = 0, hi = npos;
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (__ldg(pos + mid) <= id) lo = mid + 1;
+    else hi = mid;
+  }
+  return id + lo;
+}
+
+// Rows j0 .. j0+rows-1 of one per-node array, staged in `src`, are written to their relabelled rows of `dst`: one warp
+// per row when a row has at least 32 elements, one thread per row otherwise.
+template <class T>
+__global__ void __launch_bounds__(256) shift_rows_kernel(const T* src, T* dst, uint32_t row_elems, uint32_t j0,
+                                                         uint32_t rows, const uint32_t* pos, uint32_t npos) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool per_warp = row_elems >= 32;
+  const size_t r = per_warp ? t >> 5 : t;
+  if (r >= rows) return;
+  const size_t to = relabel_id(pos, npos, j0 + (uint32_t)r);
+  for (uint32_t c = per_warp ? (uint32_t)(t & 31) : 0; c < row_elems; c += per_warp ? 32 : 1)
+    dst[to * row_elems + c] = src[(size_t)r * row_elems + c];
+}
+
+// every stored id (adjacency entries, upper-row owners) through the relabelling; NONE stays NONE
+__global__ void relabel_ids_kernel(uint32_t* ids, size_t count, const uint32_t* pos, uint32_t npos) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  const uint32_t v = ids[i];
+  if (v != NONE) ids[i] = relabel_id(pos, npos, v);
+}
+
+// The rows of the new ids, one warp each: the vector (zero-padded to ld), an empty layer-0 row, level, first upper row,
+// alive.  Their upper rows are fresh rows at the end of adj_up.
+__global__ void place_new_rows_kernel(const uint32_t* new_ids, uint32_t count, const float* vectors, uint32_t dim,
+                                      float* vec, uint32_t ld, uint32_t* adj0, uint32_t s0, uint32_t* deg0,
+                                      const uint32_t* up_off, uint32_t* upper_off, const uint8_t* levels,
+                                      uint8_t* node_level, uint8_t* dead) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t r = t >> 5;
+  const uint32_t lane = t & 31;
+  if (r >= count) return;
+  const size_t id = new_ids[r];
+  for (uint32_t c = lane; c < ld; c += 32) vec[id * ld + c] = c < dim ? vectors[(size_t)r * dim + c] : 0.f;
+  for (uint32_t j = lane; j < s0; j += 32) adj0[id * s0 + j] = NONE;
+  if (lane == 0) {
+    deg0[id] = 0;
+    upper_off[id] = up_off[r];
+    node_level[id] = levels[r];
+    dead[id] = 0;
+  }
 }
 
 }  // namespace cozo

@@ -671,12 +671,14 @@ struct StagedHnswIndex {
   // ---- maintenance: `:put` / `:rm` on an indexed relation (query/stored.rs:332, 995-997) -------------
   // The device copy absorbs a mutation in place when dense ids can stay in compound-key order (the order
   // the entry-point rule reads, hnsw.rs:891-899): changed vectors under existing keys, removals, and new
-  // rows whose key sorts after every indexed key (the append case).  Anything else re-indexes from the
-  // base relation (`rebuilt` counts those).
+  // rows whose key sorts after every indexed key (the append case).  A new key inside the indexed range
+  // re-indexes from the base relation (`rebuilt` counts those), or, with `insert_inside`, goes to
+  // cozo_gpu_hnsw_insert_at, which moves existing ids up so that they stay in key order.
   std::map<CompoundKey, uint32_t, CompoundKeyLess> key_ids;  // compound key -> dense id (lazily rebuilt)
   std::vector<uint8_t> live;                                  // host mirror of the device's live flags
   bool is_live(uint32_t id) const { return live.size() != keys.size() || live[id] != 0; }
-  uint64_t n_put_unchanged = 0, n_put_updated = 0, n_put_appended = 0, n_removed = 0, n_rebuilt = 0;
+  uint64_t n_put_unchanged = 0, n_put_updated = 0, n_put_appended = 0, n_put_inserted = 0, n_removed = 0, n_rebuilt = 0;
+  bool insert_inside = false;  // opt-in: keys inside the indexed range are inserted in place instead of re-indexing
 
   void sync_dictionary() {
     if (key_ids.size() == keys.size() && live.size() == keys.size()) return;
@@ -779,7 +781,7 @@ struct StagedHnswIndex {
     for (const Tuple& row : rows) base.put(row);
     // a new key lands inside the indexed key range (ids must stay in key order), or nothing is indexed yet
     // (then this is create_hnsw_index over the rows just stored): re-index from the base relation
-    if (!in_order || (keys.empty() && !appended.empty())) {
+    if ((!in_order && !insert_inside) || (keys.empty() && !appended.empty())) {
       n_rebuilt++;
       build(base, manifest);
       if (filter) {
@@ -812,16 +814,46 @@ struct StagedHnswIndex {
       std::vector<float> flat;
       flat.reserve(appended.size() * dim);
       for (auto& a : appended) flat.insert(flat.end(), a.second->begin(), a.second->end());
-      uint32_t first = 0;
-      gpu_check(cozo_gpu_hnsw_insert(h, flat.data(), (uint32_t)appended.size(), 0, (uint32_t)manifest.ef_construction,
-                                     manifest.keep_pruned_connections ? 1 : 0, &first));
-      if (first != keys.size()) throw CozoError("", "device ids out of step with the key dictionary");
-      for (auto& a : appended) {
-        key_ids.emplace(a.first, (uint32_t)keys.size());
-        keys.push_back(a.first);
-        live.push_back(1);
+      const uint32_t efc = (uint32_t)manifest.ef_construction, keep = manifest.keep_pruned_connections ? 1 : 0;
+      if (in_order) {
+        uint32_t first = 0;
+        gpu_check(cozo_gpu_hnsw_insert(h, flat.data(), (uint32_t)appended.size(), 0, efc, keep, &first));
+        if (first != keys.size()) throw CozoError("", "device ids out of step with the key dictionary");
+        for (auto& a : appended) {
+          key_ids.emplace(a.first, (uint32_t)keys.size());
+          keys.push_back(a.first);
+          live.push_back(1);
+        }
+        n_put_appended += appended.size();
+      } else {
+        // position = ids (removed ones included) whose key sorts before the new key; `appended` is in key order
+        const uint32_t c = (uint32_t)appended.size();
+        std::vector<uint32_t> pos(c), ids(c);
+        for (uint32_t i = 0; i < c; ++i)
+          pos[i] = (uint32_t)(std::lower_bound(keys.begin(), keys.end(), appended[i].first, CompoundKeyLess()) - keys.begin());
+        gpu_check(cozo_gpu_hnsw_insert_at(h, pos.data(), flat.data(), c, 0, efc, keep, ids.data()));
+        std::vector<CompoundKey> k2;
+        std::vector<uint8_t> l2;
+        k2.reserve(keys.size() + c);
+        l2.reserve(keys.size() + c);
+        uint32_t j = 0;
+        for (uint32_t i = 0; i <= c; ++i) {
+          const uint32_t upto = i < c ? pos[i] : (uint32_t)keys.size();
+          for (; j < upto; ++j) {
+            k2.push_back(std::move(keys[j]));
+            l2.push_back(live[j]);
+          }
+          if (i == c) break;
+          if (ids[i] != k2.size()) throw CozoError("", "device ids out of step with the key dictionary");
+          k2.push_back(appended[i].first);
+          l2.push_back(1);
+        }
+        keys.swap(k2);
+        live.swap(l2);
+        key_ids.clear();
+        for (uint32_t i = 0; i < keys.size(); ++i) key_ids.emplace(keys[i], i);
+        n_put_inserted += c;
       }
-      n_put_appended += appended.size();
     }
   }
 

@@ -182,6 +182,7 @@ struct PyHnswIndex {
     d["put_unchanged"] = ix.n_put_unchanged;
     d["put_updated"] = ix.n_put_updated;
     d["put_appended"] = ix.n_put_appended;
+    d["put_inserted"] = ix.n_put_inserted;
     d["removed"] = ix.n_removed;
     d["rebuilt"] = ix.n_rebuilt;
     return d;
@@ -280,7 +281,10 @@ PYBIND11_MODULE(_cozo_host, m) {
       .def("put_rows", &PyHnswIndex::put_rows, py::arg("base"), py::arg("rows"), py::arg("filter") = py::none())
       .def("remove_rows", &PyHnswIndex::remove_rows)
       .def("to_index_rows", &PyHnswIndex::to_index_rows)
-      .def("info", &PyHnswIndex::info);
+      .def("info", &PyHnswIndex::info)
+      .def_property(
+          "insert_inside", [](const PyHnswIndex& p) { return p.ix.insert_inside; },
+          [](PyHnswIndex& p, bool v) { p.ix.insert_inside = v; });
   py::class_<PyHnswSearchRA>(m, "HnswSearchRA")
       .def(py::init<std::shared_ptr<PyRelation>, std::shared_ptr<PyHnswIndex>, size_t, size_t, py::object, bool, bool,
                     bool, bool, py::object, size_t, bool>(),

@@ -20,7 +20,7 @@
  *     a workspace from a bounded pool.  Graph algorithm calls are thread-safe per
  *     handle too (the staged graph is read-only, every call owns its buffers) but
  *     run on the default stream, i.e. concurrent calls serialise on the device.
- *     stage / free / build / insert / update / remove are not concurrent with
+ *     stage / free / build / insert / insert_at / update / remove are not concurrent with
  *     any other call on the same handle.
  *   - `poison` parameters point at a 32-bit flag mirroring the AtomicBool inside
  *     Poison (runtime/db.rs:1926-1942; INTEGRATION.md shows the mirror); it is
@@ -192,6 +192,18 @@ int cozo_gpu_hnsw_build(cozo_gpu_hnsw_t** out, const CozoGpuHnswBuildDesc* desc)
  * point goes, the first remaining row in key order takes over (hnsw.rs:828-865). */
 int cozo_gpu_hnsw_insert(cozo_gpu_hnsw_t* h, const float* vectors, uint32_t count, int32_t vectors_on_device,
                          uint32_t ef_construction, int32_t keep_pruned_connections, uint32_t* first_id);
+/* hnsw_put of new rows at ANY key position (query/stored.rs:332 -> hnsw.rs:679-727).
+ * positions[i] = number of ids already in the index (live or removed) whose compound key sorts before
+ * new row i; non-decreasing, <= n; rows with equal positions in key order.  Existing id j becomes
+ * j + #{i : positions[i] <= j}; new row i gets id positions[i] + i, so dense ids stay in key order.
+ * Levels come from the handle's level law, drawn in row order.  out_ids [count] nullable.
+ * Arguments and errors as cozo_gpu_hnsw_insert, plus COZO_GPU_EINVAL for positions that decrease
+ * or exceed n.  With every position equal to n the call is cozo_gpu_hnsw_insert.  After the new rows
+ * are linked, the entry point is the smallest id on the top layer (hnsw.rs:184-199).  Waits for
+ * device work already enqueued on the handle (an asynchronous search_dev) before moving rows. */
+int cozo_gpu_hnsw_insert_at(cozo_gpu_hnsw_t* h, const uint32_t* positions, const float* vectors, uint32_t count,
+                            int32_t vectors_on_device, uint32_t ef_construction,
+                            int32_t keep_pruned_connections, uint32_t* out_ids);
 int cozo_gpu_hnsw_remove(cozo_gpu_hnsw_t* h, const uint32_t* ids, uint32_t count);
 /* hnsw_put of a changed vector under an existing key (hnsw.rs:175-182: remove, then insert again);
  * vectors [count x dim] host memory, ids distinct.  The node keeps its id and layer.  Removed ids

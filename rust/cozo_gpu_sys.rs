@@ -89,6 +89,7 @@ extern "C" {
     pub fn cozo_gpu_hnsw_search_scatter_dev(h: *mut CozoGpuHnsw, queries_dev: *const f32, B: u32, k: u32, ef: u32, radius: f64, n_dest: u32, dest_ids_ptrs: *const u64, dest_dist_ptrs: *const u64, slot: u32, per_query_stats_dev: *mut u32, stream: *mut c_void) -> c_int;
     pub fn cozo_gpu_hnsw_build(out: *mut *mut CozoGpuHnsw, desc: *const CozoGpuHnswBuildDesc) -> c_int;
     pub fn cozo_gpu_hnsw_insert(h: *mut CozoGpuHnsw, vectors: *const f32, count: u32, vectors_on_device: i32, ef_construction: u32, keep_pruned_connections: i32, first_id: *mut u32) -> c_int;
+    pub fn cozo_gpu_hnsw_insert_at(h: *mut CozoGpuHnsw, positions: *const u32, vectors: *const f32, count: u32, vectors_on_device: i32, ef_construction: u32, keep_pruned_connections: i32, out_ids: *mut u32) -> c_int;
     pub fn cozo_gpu_hnsw_remove(h: *mut CozoGpuHnsw, ids: *const u32, count: u32) -> c_int;
     pub fn cozo_gpu_hnsw_update(h: *mut CozoGpuHnsw, ids: *const u32, vectors: *const f32, count: u32, ef_construction: u32, keep_pruned_connections: i32) -> c_int;
     pub fn cozo_gpu_hnsw_info(h: *mut CozoGpuHnsw, n_vectors: *mut u32, dim: *mut u32, n_levels: *mut u32, entry_point: *mut u32) -> c_int;

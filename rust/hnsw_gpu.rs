@@ -57,12 +57,50 @@ pub(crate) struct StagedIndex {
 ///   hnsw_put    <- query/stored.rs:332, :630 and runtime/relation.rs:1177 (create_hnsw_index bulk insert)
 ///   hnsw_remove <- query/stored.rs:995-997
 ///   index drop  <- runtime/relation.rs:1383 (`hnsw_indices.remove`)
-/// each calls `gpu_index_invalidate(idx_handle.id)` before touching the relation.  The next search
-/// re-stages (or, for appends and in-place updates, the glue can call cozo_gpu_hnsw_insert / _update /
-/// _remove instead — `StagedHnswIndex::put_rows` / `remove_rows` in the C++ twin show the exact rules).
+/// each calls `gpu_index_invalidate(idx_handle.id)` before touching the relation, except that a `:put` whose
+/// compound keys are all new goes through `gpu_index_put_new_keys` instead.  The next search re-stages a dropped
+/// copy (changed vectors and removals can likewise go to cozo_gpu_hnsw_update / _remove —
+/// `StagedHnswIndex::put_rows` / `remove_rows` in the C++ twin show the exact rules).
 /// A staged copy is only handed to readers whose transaction started after the staging.
 pub(crate) fn gpu_index_invalidate(idx_rel_id: crate::runtime::relation::RelationId) {
     STAGED.lock().unwrap().remove(&idx_rel_id.0);
+}
+
+/// hnsw_put of compound keys the staged copy does not hold yet, at any key position (query/stored.rs:332 ->
+/// hnsw.rs:679-727), absorbed in place by cozo_gpu_hnsw_insert_at.  `new`: (key, vector) in key order.  The device
+/// moves every existing id up by the number of new keys before it, so `keys` stays the key order the entry-point
+/// rule reads.  F64 copies (search-only on the device) and copies still shared with a reader are dropped instead:
+/// the next search re-stages them.
+pub(crate) fn gpu_index_put_new_keys(
+    idx_rel_id: crate::runtime::relation::RelationId,
+    new: &[(CompoundKey, Vec<f32>)],
+    mf: &HnswIndexManifest,
+) -> Result<()> {
+    let mut map = STAGED.lock().unwrap();
+    let Some(arc) = map.get_mut(&idx_rel_id.0) else { return Ok(()) };
+    let staged = match Arc::get_mut(arc) {
+        Some(s) if !s.f64_index => s,
+        _ => {
+            map.remove(&idx_rel_id.0);
+            return Ok(());
+        }
+    };
+    // lower_bound in the id -> key table; removed ids keep their ids (and keys) until a re-stage
+    let positions: Vec<u32> = new.iter().map(|(k, _)| staged.keys.partition_point(|x| x < k) as u32).collect();
+    let flat: Vec<f32> = new.iter().flat_map(|(_, v)| v.iter().copied()).collect();
+    let mut ids = vec![0u32; new.len()];
+    let rc = unsafe {
+        cozo_gpu_hnsw_insert_at(staged.h, positions.as_ptr(), flat.as_ptr(), new.len() as u32, 0,
+                                mf.ef_construction as u32, mf.keep_pruned_connections as i32, ids.as_mut_ptr())
+    };
+    if let Err(e) = check(rc) {
+        map.remove(&idx_rel_id.0); // the copy may be half updated: re-stage on the next search
+        return Err(e);
+    }
+    for (i, (k, _)) in new.iter().enumerate() {
+        staged.keys.insert(ids[i] as usize, k.clone()); // ids ascend: key i lands after keys 0..i
+    }
+    Ok(())
 }
 
 unsafe impl Send for StagedIndex {}
