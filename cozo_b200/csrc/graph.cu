@@ -69,6 +69,8 @@ __global__ void __launch_bounds__(256) sssp_kernel(const uint32_t* __restrict__ 
 // launch helper.  Default = the flag-scan kernel (shared-memory state when it fits).  Options, both off by default
 // because neither form has run on a GPU yet: "sssp.frontier" = 1 -> compacted frontier queues (one CTA per source),
 // "sssp.wide" = 1 -> many CTAs per source with one launch per round (host loop, capped at n + 2 rounds).
+// "sssp.smem" = 0 keeps the flag-scan state in HBM even when it fits shared memory, so that tests reach the form every
+// graph above ~23 k nodes takes with graphs small enough for exact references.
 static size_t sssp_flags_stride(uint32_t n) { return ((size_t)n * 9 + 15) & ~(size_t)15; }
 template <bool FORB>
 static cudaError_t launch_sssp(cozo_gpu_graph_t* g, const uint32_t* d_sources, uint32_t n_src,
@@ -107,7 +109,7 @@ static cudaError_t launch_sssp(cozo_gpu_graph_t* g, const uint32_t* d_sources, u
                                                    fstride, fs);
     return cudaGetLastError();
   }
-  if (need + 1024 <= di.smem_optin) {
+  if (need + 1024 <= di.smem_optin && get_option("sssp.smem", 1) != 0) {
     // raise the kernel's dynamic shared-memory limit, never lower it (concurrent callers with other graphs)
     static std::mutex mu;
     static size_t raised[2] = {0, 0};
@@ -283,7 +285,8 @@ struct CallStream {
   }
 };
 
-// shared driver of the SSSP family: runs sources in chunks that fit `budget` bytes
+// shared driver of the SSSP family: runs sources in chunks that fit `budget` bytes.  "sssp.max_chunk_sources" = k > 0
+// caps a chunk at k sources, so that tests run several chunks on small graphs.
 template <class PerChunk>
 static int sssp_chunks(cozo_gpu_graph_t* g, CallStream& cs, const uint32_t* sources_host, uint32_t n_src,
                        size_t extra_per_src, const volatile int* poison, PerChunk per_chunk) {
@@ -294,6 +297,8 @@ static int sssp_chunks(cozo_gpu_graph_t* g, CallStream& cs, const uint32_t* sour
   COZO_CUDA(cudaMemGetInfo(&freeb, &totalb));
   size_t budget = std::min<size_t>(freeb / 2, (size_t)8 << 30);
   uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(n_src, budget / std::max<size_t>(per_src, 1)));
+  const int64_t max_chunk = get_option("sssp.max_chunk_sources", 0);
+  if (max_chunk > 0) chunk = (uint32_t)std::min<int64_t>(chunk, max_chunk);
   DevBuf state, flags, dsrc;
   COZO_CUDA(cudaMalloc(&state.p, (size_t)chunk * n * 8));
   COZO_CUDA(cudaMalloc(&flags.p, (size_t)chunk * fstride));

@@ -105,9 +105,10 @@ def _pytest_on_emu(lib, args, timeout):
 
 def test_gpu_test_files_on_the_emulated_library(emu_lib):
     """the host-layer GPU tests (FixedRule / HnswSearchRA mirrors over the C ABI: PageRank, Dijkstra incl. keep_ties, Yen,
-    centralities, clustering, index build / write-back / put / rm, device filter) and the quick graph tests, unchanged,
-    with the binding pointed at libcozo_gpu_emu.so"""
-    out = _pytest_on_emu(emu_lib, ["-m", "gpu", "tests/test_host_gpu.py", "tests/test_graph_gpu.py", "-k", "not air_routes and not 17-5"], 2400)
+    centralities, clustering, index build / write-back / put / rm, device filter), the quick graph tests and the small-graph
+    exact SSSP-family tests (HBM state, several source chunks), unchanged, with the binding pointed at libcozo_gpu_emu.so"""
+    out = _pytest_on_emu(emu_lib, ["-m", "gpu", "tests/test_host_gpu.py", "tests/test_graph_gpu.py", "tests/test_graph_exact_gpu.py",
+                                   "-k", "not air_routes and not 17-5"], 2400)
     assert " passed" in out and "failed" not in out
 
 
