@@ -37,6 +37,7 @@ struct SearchParams {
   uint32_t* dest_ids[COZO_GPU_MAX_PEERS];
   float* dest_dist[COZO_GPU_MAX_PEERS];
   uint32_t off_qcodes;  // the pruned search's fixed-point query (QueryCodes::a)
+  uint32_t off_query;   // wide kernels (NV = 0): the query, zero padded to ld (per warp; per CTA in the cooperative one)
 };
 
 
@@ -143,19 +144,26 @@ __global__ void __launch_bounds__(128, MINB) hnsw_search_kernel(HnswDev g, Searc
     __syncwarp();
   }
   const int nvec4 = g.ld >> 2;
-  constexpr bool PRUNE = BULK && METRIC == COZO_GPU_L2;  // at run time: only if g.codes is set (then p.cns > 0)
+  // at run time: only if g.codes is set (then p.cns > 0); wide rows carry no codes
+  constexpr bool PRUNE = BULK && METRIC == COZO_GPU_L2 && NV > 0;
 
   for (;;) {
     uint32_t qi = 0;
     if (lane == 0) qi = atomicAdd(p.counter, 1u);
     qi = __shfl_sync(0xffffffffu, qi, 0);
     if (qi >= p.B) break;
-    float4 q[NV];
+    typename QueryOf<NV>::type q;
     float qnorm;
-    load_query<NV>(p.queries + (size_t)qi * g.dim, g.dim, lane, q, qnorm);
+    if constexpr (NV == 0)
+      load_query_wide(p.queries + (size_t)qi * g.dim, g.dim, lane, reinterpret_cast<float4*>(base + p.off_query), true,
+                      q, qnorm);
+    else
+      load_query<NV>(p.queries + (size_t)qi * g.dim, g.dim, lane, q, qnorm);
     QueryCodes qc;
     qc.a = reinterpret_cast<QueryPair*>(base + p.off_qcodes);
-    if (PRUNE && g.codes) load_query_codes<NV>(q, g.ld, lane, qc);
+    if constexpr (PRUNE) {
+      if (g.codes) load_query_codes<NV>(q, g.ld, lane, qc);
+    }
     w.len = 0;
     w.cursor = 0;
     w.dist_evals = w.nodes_expanded = w.nbr_reads = w.pruned = 0;
@@ -194,7 +202,8 @@ __global__ void __launch_bounds__(128, MINB) hnsw_search_kernel(HnswDev g, Searc
 using KernelFn = void (*)(HnswDev, SearchParams);
 
 // Cooperative form: one CTA (4 warps) per query; see coop_search_level.  Shared memory per CTA:
-// [fd ef][fi ef][pend 32][pdist 32][ctrl 8] then per warp [bars ns][ring ns rows].
+// [fd ef][fi ef][pend 32][pdist 32][ctrl 8] then per warp [bars ns][ring ns rows].  The wide form (NV = 0) keeps its
+// query between the two: [ctrl 8][query ld][per warp ...].
 template <int NV, int METRIC>
 __global__ void __launch_bounds__(128, 4) hnsw_search_coop_kernel(HnswDev g, SearchParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -234,9 +243,13 @@ __global__ void __launch_bounds__(128, 4) hnsw_search_coop_kernel(HnswDev g, Sea
     const uint32_t qi = cs.ctrl[1];
     __syncthreads();
     if (qi >= p.B) break;
-    float4 q[NV];
+    typename QueryOf<NV>::type q;
     float qnorm;
-    load_query<NV>(p.queries + (size_t)qi * g.dim, g.dim, lane, q, qnorm);
+    if constexpr (NV == 0)  // one copy per CTA, written by warp 0; every warp sums the norm itself
+      load_query_wide(p.queries + (size_t)qi * g.dim, g.dim, lane, reinterpret_cast<float4*>(smem + p.off_query),
+                      warp == 0, q, qnorm);
+    else
+      load_query<NV>(p.queries + (size_t)qi * g.dim, g.dim, lane, q, qnorm);
     w.len = 0;
     w.cursor = 0;
     w.dist_evals = w.nodes_expanded = w.nbr_reads = 0;
@@ -285,7 +298,7 @@ static KernelFn pick_coop_kernel(uint32_t ld, int metric) {
   if (need <= 6) return pick_coop_metric<6>(metric);
   if (need <= 8) return pick_coop_metric<8>(metric);
   if (need <= 16) return pick_coop_metric<16>(metric);
-  return nullptr;
+  return pick_coop_metric<0>(metric);
 }
 
 
@@ -311,7 +324,7 @@ static KernelFn pick_nv(uint32_t need, int metric, bool bulk) {
   if (need <= 6) return pick_metric<6, MINB>(metric, bulk);
   if (need <= 8) return pick_metric<8, MINB>(metric, bulk);
   if (need <= 16) return pick_metric<16, MINB>(metric, bulk);
-  return nullptr;
+  return pick_metric<0, MINB>(metric, bulk);
 }
 
 // 4 CTAs x 4 warps per SM (<= 128 registers).  The batch is bandwidth-bound; builds capped for more resident
@@ -443,12 +456,15 @@ static void codes_drop(cozo_gpu_hnsw* h) {
   h->dev.codes = nullptr;
 }
 
-// Room for `rows` code rows, keeping rows [0, n).  Only L2 f32 indexes with ld >= CODES_MIN_LD carry codes.  A failed
+// Room for `rows` code rows, keeping rows [0, n).  Only L2 f32 indexes with CODES_MIN_LD <= ld <= 2048 carry codes.  A failed
 // allocation leaves
 // the index without codes: it is then searched without pruning, with the same results.
 void hnsw_codes_reserve(cozo_gpu_hnsw* h, uint32_t rows) {
   HnswDev& g = h->dev;
-  if (h->f64 || g.metric != COZO_GPU_L2 || g.ld < CODES_MIN_LD || h->codes_failed || rows <= h->codes_rows) return;
+  // the pruning bound (hnsw_codes.cuh) is argued for ld <= REG_QUERY_MAX_LD, and the wide kernels do not prune
+  if (h->f64 || g.metric != COZO_GPU_L2 || g.ld < CODES_MIN_LD || g.ld > REG_QUERY_MAX_LD || h->codes_failed ||
+      rows <= h->codes_rows)
+    return;
   uint8_t* nc = nullptr;
   if (cudaMalloc(&nc, (size_t)rows * g.code_ld) != cudaSuccess) {
     cudaGetLastError();  // not sticky: clear it
@@ -491,46 +507,73 @@ int hnsw_launch_search(cozo_gpu_hnsw* h, HnswWorkspace* ws, const float* d_q, ui
   // the cooperative kernel wins while the batch is below about 1.5 waves of its CTAs (4 resident per SM), the
   // warp-per-query kernel beyond (tools/sweep_batch.py measures the crossover)
   const uint32_t coop_below = (uint32_t)get_option("hnsw.coop_below", (int64_t)di.sm_count * 6);
-  if (mode < 0) mode = B < coop_below ? 2 : 1;
+  const bool auto_mode = mode < 0;
+  if (auto_mode) mode = B < coop_below ? 2 : 1;
   SearchParams p{};
   uint32_t efcap = round_up(ef, 32);
   KernelFn fn = nullptr;
   uint32_t wpc = 4, grid = 0;
   size_t smem = 0;
+  // Rows wider than the register query (NV = 0 kernels) hold the query in shared memory and start from a ring of
+  // WIDE_RING_BYTES per warp; stages are dropped, down to one, only when nothing else makes the block fit.  The
+  // cooperative CTA needs the query and a stage for each of its 4 warps (up to ld ~11 500 at ef 200); the default mode
+  // takes the warp-per-query kernel (query and one stage: up to ld ~28 000) for wider rows.
+  const bool wide = g.ld > REG_QUERY_MAX_LD;
+  const uint32_t row_bytes = g.ld * 4, query_bytes = wide ? round_up(row_bytes, 128) : 0;
+  if (wide) ns = std::max<uint32_t>(1, std::min<uint32_t>(ns, WIDE_RING_BYTES / row_bytes));
+  auto wide_unsup = [&](size_t need) {
+    return set_error(COZO_GPU_EUNSUP, "vec_dim %u at ef=%u needs %zu B of shared memory (limit %zu)", g.dim, ef, need,
+                     di.smem_optin);
+  };
   if (mode == 2) {
     fn = pick_coop_kernel(g.ld, g.metric);
-    if (!fn) return set_error(COZO_GPU_EUNSUP, "vec_dim %u exceeds the supported maximum 2048", g.dim);
-    const uint32_t cns = std::min<uint32_t>(ns, 3);  // rows in flight per warp; 4 warps share a query
-    ns = cns;
+    uint32_t cns = std::min<uint32_t>(ns, 3);  // rows in flight per warp; 4 warps share a query
     p.off_fi = efcap * 4;
     p.off_pend = p.off_fi + efcap * 4;                 // pend | pdist | ctrl : 128 + 128 + 32 bytes
-    p.off_bars = round_up(p.off_pend + 288, 128);      // start of the per-warp regions
-    p.off_ring = round_up(cns * 8, 128);               // ring offset inside a warp's region
-    p.warp_smem = round_up(p.off_ring + cns * g.ld * 4, 128);
-    smem = (size_t)p.off_bars + (size_t)p.warp_smem * COOP_WARPS;
-    if (smem > di.smem_optin)
-      return set_error(COZO_GPU_EUNSUP, "ef=%u needs %zu B of shared memory per CTA (limit %zu)", ef, smem,
-                       di.smem_optin);
-    // always the device maximum: concurrent callers with different ef / stages never lower each other's limit
-    COZO_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)di.smem_optin));
-    int cps = 0;
-    COZO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cps, fn, 128, smem));
-    if (cps < 1) return set_error(COZO_GPU_ECUDA, "search kernel does not fit on an SM");
-    grid = std::min<uint32_t>((uint32_t)di.sm_count * (uint32_t)cps, B);
-    wpc = 1;  // one visited bitmap / log per CTA
-  } else {
+    p.off_query = round_up(p.off_pend + 288, 128);
+    p.off_bars = p.off_query + query_bytes;            // start of the per-warp regions
+    for (;;) {
+      p.off_ring = round_up(cns * 8, 128);               // ring offset inside a warp's region
+      p.warp_smem = round_up(p.off_ring + cns * row_bytes, 128);
+      smem = (size_t)p.off_bars + (size_t)p.warp_smem * COOP_WARPS;
+      if (smem <= di.smem_optin || !wide || cns == 1) break;
+      --cns;
+    }
+    if (smem > di.smem_optin && wide && auto_mode) {
+      mode = 1;  // the warp-per-query kernel below
+    } else {
+      ns = cns;
+      if (smem > di.smem_optin) {
+        if (wide) return wide_unsup(smem);
+        return set_error(COZO_GPU_EUNSUP, "ef=%u needs %zu B of shared memory per CTA (limit %zu)", ef, smem,
+                         di.smem_optin);
+      }
+      // always the device maximum: concurrent callers with different ef / stages never lower each other's limit
+      COZO_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)di.smem_optin));
+      int cps = 0;
+      COZO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cps, fn, 128, smem));
+      if (cps < 1) return set_error(COZO_GPU_ECUDA, "search kernel does not fit on an SM");
+      grid = std::min<uint32_t>((uint32_t)di.sm_count * (uint32_t)cps, B);
+      wpc = 1;  // one visited bitmap / log per CTA
+    }
+  }
+  if (mode != 2) {
     const bool bulk = mode != 0;
     wpc = (uint32_t)get_option("hnsw.warps_per_cta", 4);
     if (wpc < 1) wpc = 1;
     if (wpc > 4) wpc = 4;  // __launch_bounds__(128, ..)
     if (!bulk) ns = 0;
     fn = pick_kernel(g.ld, g.metric, bulk);
-    if (!fn) return set_error(COZO_GPU_EUNSUP, "vec_dim %u exceeds the supported maximum 2048", g.dim);
     p.off_fi = efcap * 4;
     p.off_pend = p.off_fi + efcap * 4;
     p.off_bars = p.off_pend + 32 * 4;
     p.off_ring = round_up(p.off_bars + ns * 8, 128);
     p.warp_smem = round_up(p.off_ring + ns * g.ld * 4, 128);
+    if (wide) {  // [fd][fi][pend][bars ns][query][ring ns]
+      p.off_query = p.off_ring;
+      p.off_ring += query_bytes;
+      p.warp_smem += query_bytes;
+    }
     if (bulk && g.codes) {
       // pruned search (prune_chunk): most rows of a hop never reach the f32 ring, so it keeps at most 2 stages and
       // the code ring takes the rest of the same per-warp budget; the CTAs resident per SM stay what they were.
@@ -553,6 +596,12 @@ int hnsw_launch_search(cozo_gpu_hnsw* h, HnswWorkspace* ws, const float* d_q, ui
       wpc >>= 1;
       smem = (size_t)p.warp_smem * wpc;
     }
+    while (wide && smem > di.smem_optin && ns > 1) {  // one warp: give up ring stages
+      --ns;
+      p.warp_smem = round_up(p.off_ring + ns * row_bytes, 128);
+      smem = p.warp_smem;
+    }
+    if (wide && smem > di.smem_optin) return wide_unsup(smem);
     if (smem > di.smem_optin)
       return set_error(COZO_GPU_EUNSUP, "ef=%u needs %zu B of shared memory per warp (limit %zu)", ef, smem,
                        di.smem_optin);

@@ -87,7 +87,7 @@ static int pick_build_kernels(const HnswDev& g, K1Fn& k1, K1Fn& k2, K4Fn& k4, Kd
   else if (need <= 6) BuildKernels<6>::get(g.metric, k1, k2, k4, kd);
   else if (need <= 8) BuildKernels<8>::get(g.metric, k1, k2, k4, kd);
   else if (need <= 16) BuildKernels<16>::get(g.metric, k1, k2, k4, kd);
-  else return set_error(COZO_GPU_EUNSUP, "vec_dim %u exceeds the supported maximum 2048", g.dim);
+  else BuildKernels<0>::get(g.metric, k1, k2, k4, kd);
   return 0;
 }
 
@@ -239,8 +239,24 @@ int hnsw_ensure_build_state(cozo_gpu_hnsw* h) {
   return 0;
 }
 
-// f32 row stages per warp of the K1 search
-static uint32_t build_stages() { return std::min(32u, std::max(1u, (uint32_t)get_option("hnsw.stages", 4))); }
+// f32 row stages per warp of the K1 search.  Wide rows start from the search's WIDE_RING_BYTES ring and give up stages,
+// down to one, while one warp (its query included) does not fit the shared-memory opt-in.
+static uint32_t build_stages(uint32_t ld, uint32_t ef_c) {
+  uint32_t ns = std::min(32u, std::max(1u, (uint32_t)get_option("hnsw.stages", 4)));
+  if (ld > REG_QUERY_MAX_LD) {
+    ns = std::max(1u, std::min(ns, WIDE_RING_BYTES / (ld * 4)));
+    while (ns > 1 && make_layout(ef_c, ns, ld).warp_bytes > device_info().smem_optin) --ns;
+  }
+  return ns;
+}
+
+// the error of a K1 layout that does not fit even one warp
+static int build_smem_unsup(const HnswDev& g, uint32_t ef_c, size_t need) {
+  if (g.ld > REG_QUERY_MAX_LD)
+    return set_error(COZO_GPU_EUNSUP, "vec_dim %u at ef_construction=%u needs %zu B of shared memory (limit %zu)", g.dim,
+                     ef_c, need, device_info().smem_optin);
+  return set_error(COZO_GPU_EUNSUP, "ef_construction=%u does not fit shared memory", ef_c);
+}
 
 // The batched insertion loop for the nodes `ids` (ascending) whose vectors, levels and upper_off are in place, linked in
 // list order.  min_entry: after each batch the entry is the smallest id on the top layer (a node inserted at a key
@@ -264,14 +280,14 @@ static int hnsw_insert_ids(cozo_gpu_hnsw* h, const std::vector<uint32_t>& ids, u
   if (extend) max_batch = 1;
   uint32_t wpc = (uint32_t)get_option("hnsw.warps_per_cta", 4);
   wpc = std::min(4u, std::max(1u, wpc));
-  const uint32_t ns = build_stages();
+  const uint32_t ns = build_stages(g.ld, ef_c);
   SmemLayout lay = make_layout(ef_c, ns, g.ld);
   size_t smem1 = (size_t)lay.warp_bytes * wpc;
   while (smem1 > di.smem_optin && wpc > 1) {
     wpc >>= 1;
     smem1 = (size_t)lay.warp_bytes * wpc;
   }
-  if (smem1 > di.smem_optin) return set_error(COZO_GPU_EUNSUP, "ef_construction=%u does not fit shared memory", ef_c);
+  if (smem1 > di.smem_optin) return build_smem_unsup(g, ef_c, smem1);
   H_CUDA(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)di.smem_optin));
   int cps = 0;
   H_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cps, k1, wpc * 32, smem1));
@@ -584,6 +600,14 @@ static int prepare_insert(cozo_gpu_hnsw* h, uint32_t ef_construction, int32_t ke
   return hnsw_ensure_build_state(h);
 }
 
+// The builder needs at least one warp's shared memory (for wide rows: query, one ring stage and the beam); an insertion
+// checks it before any row is appended or moved.
+static int check_build_smem(cozo_gpu_hnsw* h) {
+  const HnswDev& g = h->dev;
+  const uint32_t wb = make_layout(h->ef_construction, build_stages(g.ld, h->ef_construction), g.ld).warp_bytes;
+  return wb > device_info().smem_optin ? build_smem_unsup(g, h->ef_construction, wb) : 0;
+}
+
 // hnsw_put for rows that sort after every indexed key (query/stored.rs:332 -> hnsw.rs:679-727).
 extern "C" int cozo_gpu_hnsw_insert(cozo_gpu_hnsw_t* h, const float* vectors, uint32_t count, int32_t vectors_on_device,
                                     uint32_t ef_construction, int32_t keep_pruned_connections, uint32_t* first_id) {
@@ -593,6 +617,7 @@ extern "C" int cozo_gpu_hnsw_insert(cozo_gpu_hnsw_t* h, const float* vectors, ui
   if (first_id) *first_id = h->dev.n;
   if (count == 0) return 0;
   rc = prepare_insert(h, ef_construction, keep_pruned_connections);
+  if (!rc) rc = check_build_smem(h);
   if (rc) return rc;
   const uint32_t n0 = h->dev.n;
   rc = append_nodes(h, vectors, vectors_on_device, count);
@@ -664,9 +689,8 @@ extern "C" int cozo_gpu_hnsw_insert_at(cozo_gpu_hnsw_t* h, const uint32_t* posit
   }
   rc = prepare_insert(h, ef_construction, keep_pruned_connections);
   if (rc) return rc;
-  // the builder needs at least one warp's shared memory: refuse before any row moves
-  if (make_layout(h->ef_construction, build_stages(), g.ld).warp_bytes > device_info().smem_optin)
-    return set_error(COZO_GPU_EUNSUP, "ef_construction=%u does not fit shared memory", h->ef_construction);
+  rc = check_build_smem(h);  // refuse before any row moves
+  if (rc) return rc;
 
   // scratch first, so that running out of memory leaves the index as it was
   struct Scratch {
@@ -841,6 +865,7 @@ extern "C" int cozo_gpu_hnsw_update(cozo_gpu_hnsw_t* h, const uint32_t* ids, con
   if (h->ef_construction == 0) return set_error(COZO_GPU_EINVAL, "ef_construction must be set");
   if (keep_pruned_connections >= 0) h->keep_pruned = keep_pruned_connections;
   rc = hnsw_ensure_build_state(h);
+  if (!rc) rc = check_build_smem(h);
   if (rc) return rc;
   // 1. drop the old vectors' links (no-op for ids that were already removed)
   std::vector<uint32_t> live_ids;

@@ -8,6 +8,7 @@ namespace cozo {
 
 struct SmemLayout {
   uint32_t off_fi, off_pend, off_bars, off_ring, warp_bytes;
+  uint32_t off_query;  // wide rows (ld > REG_QUERY_MAX_LD): the K1 query, between the barriers and the ring
 };
 inline SmemLayout make_layout(uint32_t ef, uint32_t ns, uint32_t ld) {
   SmemLayout l;
@@ -16,8 +17,32 @@ inline SmemLayout make_layout(uint32_t ef, uint32_t ns, uint32_t ld) {
   l.off_pend = l.off_fi + efcap * 4;
   l.off_bars = l.off_pend + 32 * 4;
   l.off_ring = round_up(l.off_bars + ns * 8, 128);
+  l.off_query = l.off_ring;
+  if (ld > REG_QUERY_MAX_LD) l.off_ring += round_up(ld * 4, 128);
   l.warp_bytes = round_up(l.off_ring + ns * ld * 4, 128);
   return l;
+}
+
+// The base vector `id` of a builder task as a query: loaded into registers, or (wide) its own zero-padded row of the
+// index read in place, with the squared norm in load_query's order.
+template <int NV>
+__device__ __forceinline__ void row_query(const HnswDev& g, uint32_t id, int lane, typename QueryOf<NV>::type& q,
+                                          float& qnorm) {
+  if constexpr (NV == 0) {
+    q.v = reinterpret_cast<const float4*>(g.vec + (size_t)id * g.ld);
+    float s = 0.f;
+    for (uint32_t base = 0; base < g.ld / 4; base += 32) {  // warp-uniform, as in load_query_wide
+      if (base + lane >= g.ld / 4) continue;
+      const float4 v = q.v[base + lane];
+      s = fmaf(v.x, v.x, s);
+      s = fmaf(v.y, v.y, s);
+      s = fmaf(v.z, v.z, s);
+      s = fmaf(v.w, v.w, s);
+    }
+    qnorm = warp_sum(s);
+  } else {
+    load_query<NV>(g.vec + (size_t)id * g.ld, g.ld, lane, q, qnorm);
+  }
 }
 
 struct BuildDev {
@@ -102,9 +127,13 @@ __device__ __forceinline__ void build_search_body(const HnswDev& g, const BuildD
     const uint32_t l0 = p.coff[i];
     const uint32_t id = p.list_node[l0];
     const uint32_t lq = b.node_level[id];
-    float4 q[NV];
+    typename QueryOf<NV>::type q;
     float qnorm;
-    load_query<NV>(g.vec + (size_t)id * g.ld, g.ld, lane, q, qnorm);
+    if constexpr (NV == 0)  // the search reads its query from shared memory, like the search kernels
+      load_query_wide(g.vec + (size_t)id * g.ld, g.ld, lane, reinterpret_cast<float4*>(base + p.lay.off_query), true, q,
+                      qnorm);
+    else
+      load_query<NV>(g.vec + (size_t)id * g.ld, g.ld, lane, q, qnorm);
     float d = dist_ldg1<NV, METRIC>(q, reinterpret_cast<const float4*>(g.vec + (size_t)g.entry * g.ld), lane, nvec4,
                                     qnorm);
     if (lane == 0) {
@@ -144,9 +173,9 @@ __device__ __forceinline__ uint32_t heuristic_select(const HnswDev& g, const flo
   for (; c < cnt && ns < mm; ++c) {  // hnsw.rs:512
     const uint32_t id = cid[c] & IDMASK;
     const float dq = cd[c];
-    float4 cv[NV];
+    typename QueryOf<NV>::type cv;
     float cnorm;
-    load_query<NV>(g.vec + (size_t)id * g.ld, g.ld, lane, cv, cnorm);
+    row_query<NV>(g, id, lane, cv, cnorm);
     bool add = true;
     for (uint32_t e = 0; e < ns; ++e) {  // hnsw.rs:515-523
       float de = dist_ldg1<NV, METRIC>(cv, reinterpret_cast<const float4*>(g.vec + (size_t)sel_id[e] * g.ld), lane,
@@ -216,7 +245,7 @@ __device__ __forceinline__ void warp_bitonic_sort(unsigned long long* a, uint32_
 // Builds the extended, distance-sorted candidate list of `task` in its scratch slice; returns its length.
 // base_d / base_id: the found list (ascending); q: the base vector; self: its id.
 template <int NV, int METRIC>
-__device__ __forceinline__ uint32_t extend_candidate_list(const HnswDev& g, const BuildDev& b, const float4 (&q)[NV],
+__device__ __forceinline__ uint32_t extend_candidate_list(const HnswDev& g, const BuildDev& b, const typename QueryOf<NV>::type& q,
                                                           float qnorm, uint32_t self, uint32_t level, const float* base_d,
                                                           const uint32_t* base_id, uint32_t cnt, size_t task, int lane) {
   unsigned long long* keys = b.ext_keys + task * b.ext_cap;
@@ -328,9 +357,9 @@ __device__ __forceinline__ void build_select_body(const HnswDev& g, const BuildD
   uint32_t* cid = p.cand_id + list;
   uint32_t ccnt = p.cand_cnt[t];
   if (b.extend) {  // hnsw.rs:499-511
-    float4 q[NV];
+    typename QueryOf<NV>::type q;
     float qn;
-    load_query<NV>(g.vec + (size_t)node * g.ld, g.ld, lane, q, qn);
+    row_query<NV>(g, node, lane, q, qn);
     ccnt = extend_candidate_list<NV, METRIC>(g, b, q, qn, node, level, cd, cid, ccnt, t, lane);
     cd = b.ext_d + (size_t)t * b.ext_cap;
     cid = b.ext_id + (size_t)t * b.ext_cap;
@@ -456,9 +485,9 @@ __device__ __forceinline__ void build_link_body(const HnswDev& g, const BuildDev
     __syncwarp();
     uint32_t ns;
     if (b.extend) {  // hnsw_shrink_neighbour selects through the same routine, extension included (hnsw.rs:394-409)
-      float4 q[NV];
+      typename QueryOf<NV>::type q;
       float qn;
-      load_query<NV>(g.vec + (size_t)node * g.ld, g.ld, lane, q, qn);
+      row_query<NV>(g, node, lane, q, qn);
       const uint32_t ne = extend_candidate_list<NV, METRIC>(g, b, q, qn, node, level, s_d, s_id, nc, h, lane);
       ns = heuristic_select<NV, METRIC>(g, b.ext_d + (size_t)h * b.ext_cap, b.ext_id + (size_t)h * b.ext_cap, ne, mm,
                                         b.keep_pruned != 0, sel_id, sel_d, lane);
@@ -497,9 +526,9 @@ __global__ void __launch_bounds__(128) build_edge_dist_kernel(HnswDev g, BuildDe
     return;
   }
   const int nvec4 = g.ld >> 2;
-  float4 q[NV];
+  typename QueryOf<NV>::type q;
   float qn;
-  load_query<NV>(g.vec + (size_t)owner * g.ld, g.ld, lane, q, qn);
+  row_query<NV>(g, owner, lane, q, qn);
   uint32_t cnt = 0;
   for (uint32_t j = 0; j < stride; ++j) {
     const uint32_t t = ids[j];

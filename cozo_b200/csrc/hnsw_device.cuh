@@ -108,6 +108,110 @@ __device__ __forceinline__ float finish(float a, float b, float qnorm) {
   return (float)(1.0 - (double)a / sqrt((double)qnorm * (double)b));
 }
 
+// The register query (float4 q[NV], lane-strided) covers rows of up to 32 * 4 * 16 = 2048 floats; wider ones spill.
+// Above that the query is a WideQuery (NV = 0): a pointer to the query zero-padded to ld, which the search kernels keep
+// in shared memory and the builder's selection passes read from the index's own row.  The wide helpers below visit
+// idx = lane + 32 i in the same order as the register ones, so a wide distance is the same formula.  Their loops step
+// over warp-uniform bases with the element test inside, as the unrolled register loops do: a lane-dependent trip count
+// would put divergent control flow before the warp reductions, and ptxas keeps values across it on the stack.
+constexpr uint32_t REG_QUERY_MAX_LD = 2048;
+constexpr uint32_t WIDE_RING_BYTES = 32768;  // per-warp f32 ring budget of the wide kernels: 2 stages of 16 KB rows
+struct WideQuery {
+  const float4* v;
+};
+template <int NV>
+struct QueryOf {
+  using type = float4[NV];
+};
+template <>
+struct QueryOf<0> {
+  using type = WideQuery;
+};
+constexpr int WIDE_CHUNK = 8;  // float4 per lane and row in flight in the ld.global form
+
+template <int NV, int METRIC>
+__device__ __forceinline__ float dist_smem(const WideQuery& q, const float4* row, int lane, int nvec4, float qnorm) {
+  float a = 0.f, b = 0.f;
+#pragma unroll 4
+  for (int base = 0; base < nvec4; base += 32) {
+    const int idx = base + lane;
+    if (idx < nvec4) accum<METRIC>(q.v[idx], row[idx], a, b);
+  }
+  return finish<METRIC>(a, b, qnorm);
+}
+
+template <int NV, int METRIC>
+__device__ __forceinline__ void dist_ldg2(const WideQuery& q, const float4* r0, const float4* r1, int lane, int nvec4,
+                                          float qnorm, float& d0, float& d1) {
+  float a0 = 0.f, b0 = 0.f, a1 = 0.f, b1 = 0.f;
+  for (int base = 0; base < nvec4; base += 32 * WIDE_CHUNK) {
+    float4 v0[WIDE_CHUNK], v1[WIDE_CHUNK];
+#pragma unroll
+    for (int i = 0; i < WIDE_CHUNK; ++i) {
+      int idx = base + lane + 32 * i;
+      if (idx < nvec4) {
+        v0[i] = ldg_nc_f4(r0 + idx);
+        v1[i] = ldg_nc_f4(r1 + idx);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < WIDE_CHUNK; ++i) {
+      int idx = base + lane + 32 * i;
+      if (idx < nvec4) {
+        const float4 qv = q.v[idx];
+        accum<METRIC>(qv, v0[i], a0, b0);
+        accum<METRIC>(qv, v1[i], a1, b1);
+      }
+    }
+  }
+  d0 = finish<METRIC>(a0, b0, qnorm);
+  d1 = finish<METRIC>(a1, b1, qnorm);
+}
+
+template <int NV, int METRIC>
+__device__ __forceinline__ float dist_ldg1(const WideQuery& q, const float4* r0, int lane, int nvec4, float qnorm) {
+  float a0 = 0.f, b0 = 0.f;
+  for (int base = 0; base < nvec4; base += 32 * WIDE_CHUNK) {
+    float4 v0[WIDE_CHUNK];
+#pragma unroll
+    for (int i = 0; i < WIDE_CHUNK; ++i) {
+      int idx = base + lane + 32 * i;
+      if (idx < nvec4) v0[i] = ldg_nc_f4(r0 + idx);
+    }
+#pragma unroll
+    for (int i = 0; i < WIDE_CHUNK; ++i) {
+      int idx = base + lane + 32 * i;
+      if (idx < nvec4) accum<METRIC>(q.v[idx], v0[i], a0, b0);
+    }
+  }
+  return finish<METRIC>(a0, b0, qnorm);
+}
+
+// load_query for a wide query: zero padded to round_up(dim, 4) into `dst` (when `store`), the squared norm summed in
+// load_query's order.  Lane l writes and later reads only the elements idx = l + 32 i, so one warp needs no barrier.
+__device__ __forceinline__ void load_query_wide(const float* qp, uint32_t dim, int lane, float4* dst, bool store,
+                                                WideQuery& q, float& qnorm) {
+  float s = 0.f;
+  const uint32_t nvec4 = (dim + 3) / 4;
+  for (uint32_t base = 0; base < nvec4; base += 32) {
+    const uint32_t idx = base + lane;
+    if (idx >= nvec4) continue;
+    const uint32_t e = idx * 4;
+    float4 v;
+    v.x = qp[e];
+    v.y = e + 1 < dim ? qp[e + 1] : 0.f;
+    v.z = e + 2 < dim ? qp[e + 2] : 0.f;
+    v.w = e + 3 < dim ? qp[e + 3] : 0.f;
+    if (store) dst[idx] = v;
+    s = fmaf(v.x, v.x, s);
+    s = fmaf(v.y, v.y, s);
+    s = fmaf(v.z, v.z, s);
+    s = fmaf(v.w, v.w, s);
+  }
+  q.v = dst;
+  qnorm = warp_sum(s);
+}
+
 template <int NV, int METRIC>
 __device__ __forceinline__ float dist_smem(const float4 (&q)[NV], const float4* row, int lane, int nvec4,
                                            float qnorm) {
@@ -510,8 +614,9 @@ __device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const 
 // PRUNE (L2 with the bulk ring): when g.codes is set, the chunks of a hop that find the beam full run prune_chunk, which
 // fetches f32 rows only for the neighbours whose code row cannot rule out admission.
 // qc: the query's fixed-point form (load_query_codes), read only by prune_chunk.
+// NV = 0: the query is a WideQuery (no pruning).
 template <int NV, int METRIC, bool BULK, bool PRUNE = false>
-__device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const float4 (&q)[NV], float qnorm,
+__device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const typename QueryOf<NV>::type& q, float qnorm,
                                              uint32_t ef, uint32_t level, int lane,
                                              const QueryCodes* qc = nullptr) {
   const int nvec4 = g.ld >> 2;
@@ -571,10 +676,12 @@ __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const
       HOP_ADD(w, HC_POP, tp);
       if (!validmask) break;
       w.nbr_reads += __popc(validmask);
-      if (PRUNE && g.codes && w.len == ef) {
-        prune_chunk<NV>(g, w, q, *qc, ef, id, validmask, lane);
-        __syncwarp();
-        continue;
+      if constexpr (PRUNE) {
+        if (g.codes && w.len == ef) {
+          prune_chunk<NV>(g, w, q, *qc, ef, id, validmask, lane);
+          __syncwarp();
+          continue;
+        }
       }
       HOP_T(tv);
       uint32_t newmask;
@@ -653,7 +760,7 @@ constexpr uint32_t COOP_WARPS = 4;
 
 template <int NV, int METRIC>
 __device__ __forceinline__ void coop_search_level(const HnswDev& g, WarpCtx& w, const CoopShared& cs,
-                                                  const float4 (&q)[NV], float qnorm, uint32_t ef, uint32_t level,
+                                                  const typename QueryOf<NV>::type& q, float qnorm, uint32_t ef, uint32_t level,
                                                   int lane, int warp) {
   const int nvec4 = g.ld >> 2;
   const uint32_t row_bytes = g.ld * 4;

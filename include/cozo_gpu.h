@@ -103,7 +103,11 @@ typedef struct {
   double kernel_ms;        /* device time of the search kernel (CUDA events)   */
 } CozoGpuSearchStats;
 
-/* Builds the HBM-resident copy: padded-CSR adjacency per layer + f32 matrix. */
+/* Builds the HBM-resident copy: padded-CSR adjacency per layer + f32 matrix.  Any dim stages.  Width envelope of
+ * the f32 search, build and maintenance calls: any dim whose query (round_up(dim,4)*4 bytes), one row stage of the
+ * same size and the ef beam fit the device's shared-memory opt-in (227 KB on an H100: up to about 28 000 elements);
+ * beyond it those calls return COZO_GPU_EUNSUP naming dim, ef and the bytes needed.  (Forcing the cooperative search,
+ * option "hnsw.mode" = 2, needs a row stage per warp: up to about 11 500 elements.) */
 int cozo_gpu_hnsw_stage(cozo_gpu_hnsw_t** out, const CozoGpuHnswStageDesc* desc);
 void cozo_gpu_hnsw_free(cozo_gpu_hnsw_t* h);
 
@@ -114,7 +118,7 @@ void cozo_gpu_hnsw_free(cozo_gpu_hnsw_t* h);
  * radius < 0 means None.  With a `filter` the host passes k := ef and truncates
  * itself (hnsw.rs:943-947,997-1006).
  * out_ids [B*k] padded with COZO_GPU_NONE, out_dist [B*k] padded with +inf,
- * out_count [B] (nullable), stats nullable. */
+ * out_count [B] (nullable), stats nullable.  Widths: see cozo_gpu_hnsw_stage (EUNSUP beyond the envelope). */
 int cozo_gpu_hnsw_search(cozo_gpu_hnsw_t* h, const float* queries, uint32_t B, uint32_t k, uint32_t ef,
                          double radius, uint32_t* out_ids, float* out_dist, uint32_t* out_count,
                          CozoGpuSearchStats* stats);
@@ -179,6 +183,8 @@ typedef struct {
   uint32_t max_batch;           /* 0 = default */
 } CozoGpuHnswBuildDesc;
 
+/* Widths: the envelope of cozo_gpu_hnsw_stage with ef := ef_construction; insert, insert_at and update check it
+ * before any row is appended or moved. */
 int cozo_gpu_hnsw_build(cozo_gpu_hnsw_t** out, const CozoGpuHnswBuildDesc* desc);
 
 /* Index maintenance on the device, for an index that was built here or staged from the host.
