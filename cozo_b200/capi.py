@@ -30,6 +30,7 @@ EXPORTS = [
     "cozo_gpu_shards_unique_id", "cozo_gpu_shards_init", "cozo_gpu_shards_free", "cozo_gpu_shards_info",
     "cozo_gpu_hnsw_stage_sharded", "cozo_gpu_hnsw_search_sharded", "cozo_gpu_hnsw_search_sharded_dev",
     "cozo_gpu_hnsw_search_filtered", "cozo_gpu_hnsw_search_filtered_dev", "cozo_gpu_hnsw_search_f64",
+    "cozo_gpu_graph_stage_keys", "cozo_gpu_graph_node_endpoints", "cozo_gpu_graph_lookup_keys",
 ]
 UID_BYTES = 128
 
@@ -100,6 +101,9 @@ def load():
     L.cozo_gpu_hnsw_vectors_dev.restype = vp
     L.cozo_gpu_topk_merge_dev.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp, vp]
     L.cozo_gpu_graph_stage.argtypes = [C.POINTER(vp), u32, u64, vp, vp, vp]
+    L.cozo_gpu_graph_stage_keys.argtypes = [C.POINTER(vp), u64, vp, vp, vp, C.c_int32, vp]
+    L.cozo_gpu_graph_node_endpoints.argtypes = [vp, vp]
+    L.cozo_gpu_graph_lookup_keys.argtypes = [vp, vp, vp, u32, vp]
     L.cozo_gpu_graph_free.argtypes = [vp]
     L.cozo_gpu_graph_free.restype = None
     L.cozo_gpu_graph_export.argtypes = [vp, vp, vp, vp, vp, vp]
@@ -449,6 +453,49 @@ class Graph:
         h = C.c_void_p()
         _check(load().cozo_gpu_graph_stage(C.byref(h), n, src.size, _p(src), _p(dst), _p(w)))
         self._h = h
+
+    @staticmethod
+    def pack_keys(keys):
+        """byte strings -> (bytes u8[], offsets u64[len+1]), the layout the key calls take"""
+        keys = [bytes(k) for k in keys]
+        off = np.zeros(len(keys) + 1, np.uint64)
+        off[1:] = np.cumsum([len(k) for k in keys], dtype=np.uint64)
+        return np.frombuffer(b"".join(keys) or b"\0", np.uint8).copy(), off
+
+    @classmethod
+    def from_keys(cls, key_bytes, key_off=None, w=None, undirected=False):
+        """Stage from node KEYS: endpoint 2e is edge e's from key, 2e+1 its to key.  `key_bytes` is a list of 2m byte
+        strings, or (with `key_off` [2m+1]) one u8 buffer.  Dense ids in first-appearance order; undirected mirrors
+        every edge right after itself."""
+        if key_off is None:
+            key_bytes, key_off = cls.pack_keys(key_bytes)
+        key_bytes = np.ascontiguousarray(key_bytes, np.uint8)
+        key_off = np.ascontiguousarray(key_off, np.uint64)
+        m = (key_off.size - 1) // 2
+        w = None if w is None else np.ascontiguousarray(w, np.float32)
+        g = cls.__new__(cls)
+        h, n = C.c_void_p(), C.c_uint32()
+        _check(load().cozo_gpu_graph_stage_keys(C.byref(h), m, _p(key_bytes), _p(key_off), _p(w), int(bool(undirected)),
+                                                C.byref(n)))
+        g._h = h
+        g.n, g.m, g.weighted = n.value, 2 * m if undirected else m, w is not None
+        return g
+
+    def node_endpoints(self):
+        """per dense id, the endpoint index where its key first appeared (graphs staged from keys)"""
+        out = np.zeros(max(self.n, 1), np.uint64)
+        _check(load().cozo_gpu_graph_node_endpoints(self._h, _p(out)))
+        return out[:self.n]
+
+    def lookup_keys(self, key_bytes, key_off=None):
+        """dense id of every key (list of byte strings, or buffer + offsets); NONE where the graph has no such node"""
+        if key_off is None:
+            key_bytes, key_off = self.pack_keys(key_bytes)
+        key_bytes = np.ascontiguousarray(key_bytes, np.uint8)
+        key_off = np.ascontiguousarray(key_off, np.uint64)
+        out = np.zeros(max(key_off.size - 1, 1), np.uint32)
+        _check(load().cozo_gpu_graph_lookup_keys(self._h, _p(key_bytes), _p(key_off), key_off.size - 1, _p(out)))
+        return out[:key_off.size - 1]
 
     def export(self):
         out_ptr = np.zeros(self.n + 1, np.uint32)

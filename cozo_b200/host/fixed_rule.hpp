@@ -21,6 +21,7 @@
 
 #include "../../include/cozo_gpu.h"
 #include "data_value.hpp"
+#include "memcmp.hpp"
 
 namespace cozo_host {
 
@@ -56,6 +57,14 @@ struct RegularTempStore {
   }
 };
 
+// the first field of every non-empty row: the node keys of a starting / termination relation
+inline std::vector<const DataValue*> first_fields(const std::vector<Tuple>& rows) {
+  std::vector<const DataValue*> out;
+  for (const Tuple& t : rows)
+    if (!t.empty()) out.push_back(&t[0]);
+  return out;
+}
+
 inline void gpu_check(int rc) {
   if (rc == COZO_GPU_OK) return;
   const char* msg = cozo_gpu_last_error();
@@ -63,16 +72,37 @@ inline void gpu_check(int rc) {
   throw CozoError("gpu::error", std::string("cozo_gpu error ") + std::to_string(rc) + ": " + (msg ? msg : ""));
 }
 
-// The dense-id graph handed to the device: what GraphBuilder::edges / edges_with_values
-// receives (fixed_rule/mod.rs:192-195, 318-321), before CSR construction on the device.
+// The graph on the device: what GraphBuilder::edges / edges_with_values receives (fixed_rule/mod.rs:192-195,
+// 318-321) after cozo_gpu_graph_stage_keys assigned the dense ids, plus the id -> key table.
 struct StagedGraph {
   cozo_gpu_graph_t* g = nullptr;
-  std::vector<DataValue> indices;                            // id -> key
-  std::map<DataValue, uint32_t, DataValueLess> inv_indices;  // key -> id
+  std::vector<DataValue> indices;  // id -> key
+  uint64_t n_edges = 0;            // after mirroring
   uint32_t node_count() const { return (uint32_t)indices.size(); }
-  // host copy of the edge stream (needed for keep_ties path enumeration)
-  std::vector<uint32_t> src, dst;
-  std::vector<float> w;
+  // key -> id, COZO_GPU_NONE where the graph has no such node (cozo_gpu_graph_lookup_keys on memcmp encodings)
+  std::vector<uint32_t> lookup(const std::vector<const DataValue*>& keys) const {
+    std::string kb;
+    std::vector<uint64_t> ko{0};
+    for (const DataValue* k : keys) {
+      memcmp_codec::encode_datavalue(kb, *k);
+      ko.push_back(kb.size());
+    }
+    std::vector<uint32_t> ids(keys.size());
+    if (!keys.empty())
+      gpu_check(cozo_gpu_graph_lookup_keys(g, reinterpret_cast<const uint8_t*>(kb.data()), ko.data(),
+                                           (uint32_t)keys.size(), ids.data()));
+    return ids;
+  }
+  // the dense edge stream read back in out-CSR order: by (src, dst), parallel edges in input order
+  void edges(std::vector<uint32_t>& src, std::vector<uint32_t>& dst, std::vector<float>& w) const {
+    std::vector<uint32_t> ptr((size_t)node_count() + 1);
+    src.resize(n_edges);
+    dst.resize(n_edges);
+    w.resize(n_edges);
+    gpu_check(cozo_gpu_graph_export(g, ptr.data(), dst.data(), w.data(), nullptr, nullptr));
+    for (uint32_t u = 0; u < node_count(); ++u)
+      for (uint32_t e = ptr[u]; e < ptr[u + 1]; ++e) src[e] = u;
+  }
   StagedGraph() = default;
   StagedGraph(const StagedGraph&) = delete;
   StagedGraph& operator=(const StagedGraph&) = delete;
@@ -96,22 +126,18 @@ struct FixedRuleInputRelation {
 
   // as_directed_graph (mod.rs:136-200) / as_directed_weighted_graph (mod.rs:208-328)
   void as_graph(bool undirected, bool weighted, bool allow_negative_weights, StagedGraph& out) const {
-    auto id_of = [&](const DataValue& k) -> uint32_t {  // first-appearance order (mod.rs:164-179)
-      auto it = out.inv_indices.find(k);
-      if (it != out.inv_indices.end()) return it->second;
-      uint32_t idx = (uint32_t)out.indices.size();
-      out.inv_indices.emplace(k, idx);
-      out.indices.push_back(k);
-      return idx;
-    };
+    // endpoint keys as memcmp encodings (data/memcmp.rs: equal bytes <=> equal values); the device assigns the dense
+    // ids in first-appearance order (mod.rs:164-179)
+    std::string kb;
+    std::vector<uint64_t> ko{0};
+    std::vector<float> w;
+    ko.reserve(tuples->size() * 2 + 1);
     std::unique_ptr<CozoError> error;  // the reference records the error and keeps scanning
     for (const Tuple& t : *tuples) {
       if (t.size() < 2) {  // mod.rs:150-163
         error.reset(new CozoError("algo::not_an_edge", "The relation cannot be interpreted as an edge"));
         continue;
       }
-      uint32_t f = id_of(t[0]);
-      uint32_t to = id_of(t[1]);
       float wv = 1.0f;  // mod.rs:254-255
       if (weighted && t.size() >= 3) {
         double x;
@@ -122,18 +148,23 @@ struct FixedRuleInputRelation {
         }
         wv = (float)x;  // mod.rs:306
       }
-      out.src.push_back(f);
-      out.dst.push_back(to);
-      if (weighted) out.w.push_back(wv);
-      if (undirected) {  // mod.rs:187-191, 313-317
-        out.src.push_back(to);
-        out.dst.push_back(f);
-        if (weighted) out.w.push_back(wv);
-      }
+      memcmp_codec::encode_datavalue(kb, t[0]);
+      ko.push_back(kb.size());
+      memcmp_codec::encode_datavalue(kb, t[1]);
+      ko.push_back(kb.size());
+      if (weighted) w.push_back(wv);
     }
     if (error) throw *error;
-    gpu_check(cozo_gpu_graph_stage(&out.g, out.node_count(), out.src.size(), out.src.data(), out.dst.data(),
-                                   weighted ? out.w.data() : nullptr));
+    // no error: edge e is tuple e, so endpoint i is field i % 2 of tuple i / 2
+    const uint64_t m = (ko.size() - 1) / 2;
+    uint32_t n = 0;
+    gpu_check(cozo_gpu_graph_stage_keys(&out.g, m, reinterpret_cast<const uint8_t*>(kb.data()), ko.data(),
+                                        weighted ? w.data() : nullptr, undirected ? 1 : 0, &n));
+    out.n_edges = undirected ? 2 * m : m;  // mod.rs:187-191, 313-317 (mirrored on the device)
+    std::vector<uint64_t> first(n);
+    gpu_check(cozo_gpu_graph_node_endpoints(out.g, first.data()));
+    out.indices.reserve(n);
+    for (uint64_t ep : first) out.indices.push_back((*tuples)[ep / 2][ep % 2]);
   }
   void as_directed_graph(bool undirected, StagedGraph& out) const { as_graph(undirected, false, false, out); }
   void as_directed_weighted_graph(bool undirected, bool allow_negative_weights, StagedGraph& out) const {
@@ -311,19 +342,13 @@ struct ShortestPathDijkstra : FixedRule {
     StagedGraph g;
     edges.as_directed_weighted_graph(undirected, false, g);
     std::set<uint32_t> starting_nodes;  // BTreeSet, :47-54
-    for (const Tuple& t : starting.iter()) {
-      if (t.empty()) continue;
-      auto it = g.inv_indices.find(t[0]);
-      if (it != g.inv_indices.end()) starting_nodes.insert(it->second);
-    }
+    for (uint32_t id : g.lookup(first_fields(starting.iter())))
+      if (id != COZO_GPU_NONE) starting_nodes.insert(id);
     bool has_term = payload.has_input(2);  // `termination` is optional, :41,55-68
     std::set<uint32_t> termination_nodes;
     if (has_term)
-      for (const Tuple& t : payload.get_input(2).iter()) {
-        if (t.empty()) continue;
-        auto it = g.inv_indices.find(t[0]);
-        if (it != g.inv_indices.end()) termination_nodes.insert(it->second);
-      }
+      for (uint32_t id : g.lookup(first_fields(payload.get_input(2).iter())))
+        if (id != COZO_GPU_NONE) termination_nodes.insert(id);
     if (starting_nodes.empty()) return;
     const uint32_t n = g.node_count();
     std::vector<uint32_t> sources(starting_nodes.begin(), starting_nodes.end());
@@ -335,8 +360,11 @@ struct ShortestPathDijkstra : FixedRule {
     const bool ties = keep_ties && has_term;
     std::vector<std::vector<std::pair<uint32_t, float>>> in_edges;
     if (ties) {
+      std::vector<uint32_t> es, ed;
+      std::vector<float> ew;
+      g.edges(es, ed, ew);
       in_edges.resize(n);
-      for (size_t e = 0; e < g.src.size(); ++e) in_edges[g.dst[e]].push_back({g.src[e], g.w[e]});
+      for (size_t e = 0; e < es.size(); ++e) in_edges[ed[e]].push_back({es[e], ew[e]});
     }
     // an empty termination set means "already exhausted": the search stops after the start
     // node and the goal iterator is empty (Goal for BTreeSet, :260-272) => no rows.
@@ -511,16 +539,10 @@ struct KShortestPathYen : FixedRule {
     StagedGraph g;
     edges.as_directed_weighted_graph(undirected, false, g);
     std::set<uint32_t> starts, goals;  // BTreeSets, yen.rs:43-58
-    for (const Tuple& t : starting.iter())
-      if (!t.empty()) {
-        auto it = g.inv_indices.find(t[0]);
-        if (it != g.inv_indices.end()) starts.insert(it->second);
-      }
-    for (const Tuple& t : termination.iter())
-      if (!t.empty()) {
-        auto it = g.inv_indices.find(t[0]);
-        if (it != g.inv_indices.end()) goals.insert(it->second);
-      }
+    for (uint32_t id : g.lookup(first_fields(starting.iter())))
+      if (id != COZO_GPU_NONE) starts.insert(id);
+    for (uint32_t id : g.lookup(first_fields(termination.iter())))
+      if (id != COZO_GPU_NONE) goals.insert(id);
     std::vector<PairState> ps;
     for (uint32_t s0 : starts)
       for (uint32_t g0 : goals) {
@@ -530,9 +552,15 @@ struct KShortestPathYen : FixedRule {
         ps.push_back(std::move(p));
       }
     if (ps.empty()) return;
-    // first edge s->d in adjacency order supplies the root-path cost (yen.rs:171-183)
+    // first edge s->d in adjacency order supplies the root-path cost (yen.rs:171-183); the CSR keeps parallel edges
+    // in input order
     std::map<std::pair<uint32_t, uint32_t>, float> first_edge;
-    for (size_t e = 0; e < g.src.size(); ++e) first_edge.emplace(std::make_pair(g.src[e], g.dst[e]), g.w[e]);
+    {
+      std::vector<uint32_t> es, ed;
+      std::vector<float> ew;
+      g.edges(es, ed, ew);
+      for (size_t e = 0; e < es.size(); ++e) first_edge.emplace(std::make_pair(es[e], ed[e]), ew[e]);
+    }
 
     std::vector<Search> batch;
     std::vector<std::pair<float, std::vector<uint32_t>>> res;

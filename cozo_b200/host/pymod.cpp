@@ -459,7 +459,76 @@ PYBIND11_MODULE(_cozo_host, m) {
     d["index_rows_per_s"] = (double)ikv.kv.size() / s;
     return d;
   });
-  m.def("relation_to_kv", [](const PyRelation& rel, uint64_t id) {
+  // Node id assignment of as_directed_graph on the host, the way it ran before the device took it over: a
+  // std::map<DataValue, u32> lookup per endpoint in first-appearance order (fixed_rule/mod.rs:164-179).  Also times the
+  // memcmp encoding of the same endpoints that cozo_gpu_graph_stage_keys receives instead, and returns it.
+  // `keys`: the 2m endpoint keys, an int64 numpy array (Int values, built on the fly) or any sequence of values.
+  m.def("bench_id_assign", [](py::object keys, bool run_map) {
+    std::vector<DataValue> vals;
+    py::array_t<int64_t> ints;
+    const bool is_int = py::isinstance<py::array>(keys) && py::array(keys).dtype().kind() == 'i';
+    if (is_int) ints = py::array_t<int64_t, py::array::c_style | py::array::forcecast>::ensure(keys);
+    else vals = to_tuple(keys);
+    const size_t E = is_int ? (size_t)ints.size() : vals.size();
+    const int64_t* ip = is_int ? ints.data() : nullptr;
+    auto key = [&](size_t i) { return is_int ? DataValue::from_int(ip[i]) : vals[i]; };
+    py::dict d;
+    d["endpoints"] = E;
+    d["map_s"] = py::none();
+    if (run_map) {
+      auto t0 = std::chrono::steady_clock::now();
+      std::map<DataValue, uint32_t, DataValueLess> inv;
+      std::vector<DataValue> indices;
+      std::vector<uint32_t> ids(E);
+      for (size_t i = 0; i < E; ++i) {
+        DataValue k = key(i);
+        auto it = inv.find(k);
+        if (it != inv.end()) {
+          ids[i] = it->second;
+          continue;
+        }
+        ids[i] = (uint32_t)indices.size();
+        inv.emplace(k, ids[i]);
+        indices.push_back(std::move(k));
+      }
+      d["map_s"] = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+      d["distinct"] = indices.size();
+    }
+    auto t0 = std::chrono::steady_clock::now();
+    std::string kb;
+    py::array_t<uint64_t> ko(E + 1);
+    uint64_t* o = ko.mutable_data();
+    o[0] = 0;
+    for (size_t i = 0; i < E; ++i) {
+      memcmp_codec::encode_datavalue(kb, key(i));
+      o[i + 1] = kb.size();
+    }
+    d["encode_s"] = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    py::array_t<uint8_t> kba(std::max<size_t>(kb.size(), 1));
+    std::copy(kb.begin(), kb.end(), kba.mutable_data());
+    d["key_bytes"] = kba;
+    d["key_off"] = ko;
+    return d;
+  }, py::arg("keys"), py::arg("run_map") = true);
+  // a graph rule end to end through the host mirror on Int-keyed edges (rows built here, not timed):
+  // as_graph's scan + encoding + device staging + the rule + the RegularTempStore fill
+  m.def("bench_rule_int_edges", [](const std::string& name, py::array_t<int64_t, py::array::c_style | py::array::forcecast> src,
+                                   py::array_t<int64_t, py::array::c_style | py::array::forcecast> dst, py::dict options) {
+    std::vector<std::vector<Tuple>> ins(1);
+    ins[0].reserve(src.size());
+    for (ssize_t e = 0; e < src.size(); ++e)
+      ins[0].push_back({DataValue::from_int(src.data()[e]), DataValue::from_int(dst.data()[e])});
+    Options opts;
+    for (auto kv : options) opts[kv.first.cast<std::string>()] = to_dv(kv.second);
+    FixedRuleRegistry reg;
+    auto t0 = std::chrono::steady_clock::now();
+    std::vector<Tuple> rows = reg.run(name, ins, {2}, std::move(opts), 0, Poison());
+    py::dict d;
+    d["seconds"] = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    d["rows"] = rows.size();
+    return d;
+  });
+  m.def("relation_to_kv",[](const PyRelation& rel, uint64_t id) {
     KvRelation r = KvRelation::encode(rel.rel, id);
     py::list out;
     for (auto& kv : r.kv) out.append(py::make_tuple(py::bytes(kv.first), py::bytes(kv.second)));

@@ -12,9 +12,10 @@
  *     is available from cozo_gpu_last_error() (thread-local).
  *   - pointers are caller-owned HOST memory unless the parameter / function name
  *     says `_dev` (device memory on the current device).
- *   - ids are dense u32 assigned by the host (Rust) side, which keeps the
- *     id <-> (Tuple key, field, sub-index) table (CompoundKey, hnsw.rs:55) or the
- *     id <-> DataValue table (fixed_rule/mod.rs:144-145).
+ *   - ids are dense u32.  HNSW ids are assigned by the host (Rust) side, which keeps the
+ *     id <-> (Tuple key, field, sub-index) table (CompoundKey, hnsw.rs:55); graph node ids
+ *     are assigned by the host too (cozo_gpu_graph_stage) or on the device from the node
+ *     keys' memcmp encodings (cozo_gpu_graph_stage_keys), fixed_rule/mod.rs:144-179.
  *   - there is NO CPU fallback: without a usable sm_90 device init fails.
  *   - search calls are re-entrant per handle: each call takes its own stream and
  *     a workspace from a bounded pool.  Graph algorithm calls are thread-safe per
@@ -285,6 +286,24 @@ typedef struct cozo_gpu_graph cozo_gpu_graph_t;
 int cozo_gpu_graph_stage(cozo_gpu_graph_t** out, uint32_t n, uint64_t m, const uint32_t* src,
                          const uint32_t* dst, const float* w_or_null);
 void cozo_gpu_graph_free(cozo_gpu_graph_t* g);
+/* as_directed_graph / as_directed_weighted_graph (fixed_rule/mod.rs:136-328) from node KEYS.
+ * Endpoint 2e is the `from` key of edge e, endpoint 2e+1 its `to` key, as the byte string
+ * key_bytes[key_off[i] .. key_off[i+1]) (key_off [2m+1], non-decreasing).  Two keys are the same
+ * node iff their byte strings are equal (the host passes memcmp encodings, data/memcmp.rs).
+ * Dense ids are assigned in first-appearance order over endpoints 0, 1, 2, ... (mod.rs:164-179);
+ * *out_n = number of distinct keys.  undirected != 0 mirrors every edge right after itself
+ * (mod.rs:187-191).  Weights and the CSR: exactly as cozo_gpu_graph_stage, so the handle is one
+ * every graph call takes.  COZO_GPU_EINVAL for decreasing offsets or a null pointer when m > 0;
+ * COZO_GPU_EUNSUP beyond 2^32-2 edges after mirroring (or 2^31-2 edges before it); COZO_GPU_ENOMEM
+ * when the device cannot hold the work, with the bytes needed in the message. */
+int cozo_gpu_graph_stage_keys(cozo_gpu_graph_t** out, uint64_t m, const uint8_t* key_bytes,
+                              const uint64_t* key_off, const float* w_or_null, int32_t undirected,
+                              uint32_t* out_n);
+/* for every dense id, the endpoint index (2e or 2e+1) where its key first appeared: out_first [n] */
+int cozo_gpu_graph_node_endpoints(cozo_gpu_graph_t* g, uint64_t* out_first);
+/* dense id of each key (same byte form), COZO_GPU_NONE where the graph has no such node */
+int cozo_gpu_graph_lookup_keys(cozo_gpu_graph_t* g, const uint8_t* key_bytes, const uint64_t* key_off,
+                               uint32_t count, uint32_t* out_ids);
 /* read the staged CSR back (any pointer nullable): out_ptr/in_ptr [n+1] u32 */
 int cozo_gpu_graph_export(cozo_gpu_graph_t* g, uint32_t* out_ptr, uint32_t* out_idx, float* out_w,
                           uint32_t* in_ptr, uint32_t* in_idx);

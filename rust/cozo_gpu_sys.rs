@@ -108,6 +108,9 @@ extern "C" {
     pub fn cozo_gpu_hnsw_search_sharded_dev(s: *mut CozoGpuShards, queries_dev: *const f32, B: u32, k: u32, ef: u32, radius: f64, out_ids_dev: *mut u64, out_dist_dev: *mut f32, per_query_stats_dev: *mut u32, stream: *mut c_void) -> c_int;
     pub fn cozo_gpu_graph_stage(out: *mut *mut CozoGpuGraph, n: u32, m: u64, src: *const u32, dst: *const u32, w_or_null: *const f32) -> c_int;
     pub fn cozo_gpu_graph_free(g: *mut CozoGpuGraph);
+    pub fn cozo_gpu_graph_stage_keys(out: *mut *mut CozoGpuGraph, m: u64, key_bytes: *const u8, key_off: *const u64, w_or_null: *const f32, undirected: i32, out_n: *mut u32) -> c_int;
+    pub fn cozo_gpu_graph_node_endpoints(g: *mut CozoGpuGraph, out_first: *mut u64) -> c_int;
+    pub fn cozo_gpu_graph_lookup_keys(g: *mut CozoGpuGraph, key_bytes: *const u8, key_off: *const u64, count: u32, out_ids: *mut u32) -> c_int;
     pub fn cozo_gpu_graph_export(g: *mut CozoGpuGraph, out_ptr: *mut u32, out_idx: *mut u32, out_w: *mut f32, in_ptr: *mut u32, in_idx: *mut u32) -> c_int;
     pub fn cozo_gpu_pagerank(g: *mut CozoGpuGraph, damping: f32, tol: f64, max_iter: u32, out_scores: *mut f32, out_iters: *mut u32, out_err: *mut f64, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
     pub fn cozo_gpu_sssp_multi(g: *mut CozoGpuGraph, sources: *const u32, n_src: u32, out_dist: *mut f32, out_pred: *mut u32, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;

@@ -7,9 +7,9 @@
 //! tests drive.
 //!
 //! What stays host-side, exactly as in the reference: option parsing (FixedRulePayload getters),
-//! the DataValue <-> dense-id dictionary (first-appearance order, fixed_rule/mod.rs:136-300), and
-//! the emission of result tuples into RegularTempStore.  What moves: CSR construction and the
-//! algorithm itself.
+//! the tuple scan with its arity / weight checks, the memcmp encoding of the node keys, and
+//! the emission of result tuples into RegularTempStore.  What moves: dense id assignment
+//! (fixed_rule/mod.rs:164-179), CSR construction and the algorithm itself.
 
 use std::collections::{BTreeMap, BTreeSet};
 use std::os::raw::c_int;
@@ -20,6 +20,7 @@ use miette::{bail, miette, Result};
 use smartstring::{LazyCompact, SmartString};
 
 use crate::data::expr::Expr;
+use crate::data::memcmp::MemCmpEncoder;
 use crate::data::symb::Symbol;
 use crate::data::value::DataValue;
 use crate::fixed_rule::{FixedRule, FixedRuleInputRelation, FixedRulePayload};
@@ -117,91 +118,107 @@ impl Drop for PoisonMirror {
     }
 }
 
-/// The edge list of an input relation in dense ids — the part of `as_directed_graph` /
-/// `as_directed_weighted_graph` (fixed_rule/mod.rs:136-300) that precedes `GraphBuilder`, which
-/// the device replaces (CUB radix sort, graph.cu).  Dictionary order = first appearance, `from`
-/// before `to`, so `indices` is identical to the reference's.
+/// An input relation staged on the device as a graph — `as_directed_graph` /
+/// `as_directed_weighted_graph` (fixed_rule/mod.rs:136-328).  The host scans the tuples, checks
+/// arity and weights with the reference's error precedence, and memcmp-encodes every endpoint key
+/// (data/memcmp.rs: equal bytes <=> equal values); the device assigns the dense ids in first-appearance
+/// order, `from` before `to`, and builds the CSR (cozo_gpu_graph_stage_keys, graph.cu).  So
+/// `indices` is identical to the reference's and no BTreeMap is built.
 pub(crate) struct EdgeList {
-    pub src: Vec<u32>,
-    pub dst: Vec<u32>,
-    pub w: Option<Vec<f32>>,
+    pub g: DevGraph,
     pub indices: Vec<DataValue>,
-    pub inv_indices: BTreeMap<DataValue, u32>,
+    /// after mirroring
+    pub n_edges: usize,
 }
 
 impl<'a, 'b> FixedRuleInputRelation<'a, 'b> {
     pub(crate) fn as_edge_list(&self, undirected: bool, weighted: bool) -> Result<EdgeList> {
-        let mut el = EdgeList {
-            src: vec![],
-            dst: vec![],
-            w: if weighted { Some(vec![]) } else { None },
-            indices: vec![],
-            inv_indices: Default::default(),
-        };
+        let mut tuples = vec![];
+        let mut key_bytes: Vec<u8> = vec![];
+        let mut key_off: Vec<u64> = vec![0];
+        let mut w: Vec<f32> = vec![];
         for tuple in self.iter()? {
             let tuple = tuple?;
-            let mut it = tuple.into_iter();
-            let from = it.next().ok_or_else(|| crate::fixed_rule::NotAnEdgeError(self.span()))?;
-            let to = it.next().ok_or_else(|| crate::fixed_rule::NotAnEdgeError(self.span()))?;
-            let mut id_of = |v: DataValue| -> u32 {
-                if let Some(i) = el.inv_indices.get(&v) {
-                    *i
-                } else {
-                    let i = el.indices.len() as u32;
-                    el.inv_indices.insert(v.clone(), i);
-                    el.indices.push(v);
-                    i
-                }
-            };
-            let f = id_of(from);
-            let t = id_of(to);
+            if tuple.len() < 2 {
+                bail!(crate::fixed_rule::NotAnEdgeError(self.span()));
+            }
             let mut wt = 1.0f32;
             if weighted {
-                if let Some(d) = it.next() {
+                if let Some(d) = tuple.get(2) {
                     // fixed_rule/mod.rs:243-290: non-numeric, non-finite and negative weights are errors
                     match d.get_float() {
                         Some(x) if x.is_finite() && x >= 0. => wt = x as f32,
-                        _ => bail!(crate::fixed_rule::BadEdgeWeightError(d, self.span())),
+                        _ => bail!(crate::fixed_rule::BadEdgeWeightError(d.clone(), self.span())),
                     }
                 }
             }
-            el.src.push(f);
-            el.dst.push(t);
-            if let Some(w) = el.w.as_mut() {
+            key_bytes.encode_datavalue(&tuple[0]);
+            key_off.push(key_bytes.len() as u64);
+            key_bytes.encode_datavalue(&tuple[1]);
+            key_off.push(key_bytes.len() as u64);
+            if weighted {
                 w.push(wt);
             }
-            if undirected {
-                el.src.push(t);
-                el.dst.push(f);
-                if let Some(w) = el.w.as_mut() {
-                    w.push(wt);
-                }
+            tuples.push(tuple);
+        }
+        ensure_device()?;
+        let m = tuples.len() as u64;
+        let mut g: *mut CozoGpuGraph = ptr::null_mut();
+        let mut n = 0u32;
+        check(unsafe {
+            cozo_gpu_graph_stage_keys(
+                &mut g, m, key_bytes.as_ptr(), key_off.as_ptr(),
+                if weighted { w.as_ptr() } else { ptr::null() },
+                undirected as i32, &mut n,
+            )
+        })?;
+        let g = DevGraph(g);
+        let mut first = vec![0u64; n as usize];
+        check(unsafe { cozo_gpu_graph_node_endpoints(g.0, first.as_mut_ptr()) })?;
+        // endpoint i is field i % 2 of edge (= tuple) i / 2
+        let indices = first.iter().map(|&ep| tuples[(ep / 2) as usize][(ep % 2) as usize].clone()).collect();
+        Ok(EdgeList { g, indices, n_edges: if undirected { 2 * m as usize } else { m as usize } })
+    }
+}
+
+impl EdgeList {
+    /// dense id of the first field of every row of `rel` that the graph has (starting / goal nodes)
+    fn lookup_first_fields(&self, rel: &FixedRuleInputRelation<'_, '_>) -> Result<Vec<u32>> {
+        let mut key_bytes: Vec<u8> = vec![];
+        let mut key_off: Vec<u64> = vec![0];
+        for t in rel.iter()? {
+            key_bytes.encode_datavalue(&t?[0]);
+            key_off.push(key_bytes.len() as u64);
+        }
+        let count = key_off.len() - 1;
+        let mut ids = vec![COZO_GPU_NONE; count];
+        if count > 0 {
+            check(unsafe {
+                cozo_gpu_graph_lookup_keys(self.g.0, key_bytes.as_ptr(), key_off.as_ptr(), count as u32, ids.as_mut_ptr())
+            })?;
+        }
+        Ok(ids.into_iter().filter(|&i| i != COZO_GPU_NONE).collect())
+    }
+    /// the dense edge stream in out-CSR order: by (src, dst), parallel edges in input order
+    fn edges(&self) -> Result<(Vec<u32>, Vec<u32>, Vec<f32>)> {
+        let n = self.indices.len();
+        let mut ptr_ = vec![0u32; n + 1];
+        let (mut dst, mut w) = (vec![0u32; self.n_edges], vec![0f32; self.n_edges]);
+        check(unsafe {
+            cozo_gpu_graph_export(self.g.0, ptr_.as_mut_ptr(), dst.as_mut_ptr(), w.as_mut_ptr(), ptr::null_mut(), ptr::null_mut())
+        })?;
+        let mut src = vec![0u32; self.n_edges];
+        for u in 0..n {
+            for e in ptr_[u]..ptr_[u + 1] {
+                src[e as usize] = u as u32;
             }
         }
-        Ok(el)
+        Ok((src, dst, w))
     }
 }
 
 /// RAII handle of a staged graph.
-struct DevGraph(*mut CozoGpuGraph);
-
-impl DevGraph {
-    fn stage(el: &EdgeList) -> Result<Self> {
-        ensure_device()?;
-        let mut g: *mut CozoGpuGraph = ptr::null_mut();
-        check(unsafe {
-            cozo_gpu_graph_stage(
-                &mut g,
-                el.indices.len() as u32,
-                el.src.len() as u64,
-                el.src.as_ptr(),
-                el.dst.as_ptr(),
-                el.w.as_ref().map_or(ptr::null(), |w| w.as_ptr()),
-            )
-        })?;
-        Ok(Self(g))
-    }
-}
+pub(crate) struct DevGraph(*mut CozoGpuGraph);
 
 impl Drop for DevGraph {
     fn drop(&mut self) {
@@ -226,7 +243,7 @@ impl FixedRule for PageRankGpu {
         if el.indices.is_empty() {
             return Ok(());
         }
-        let g = DevGraph::stage(&el)?;
+        let g = &el.g;
         let pm = PoisonMirror::new(poison);
         let mut ranks = vec![0f32; el.indices.len()];
         let (mut iters, mut err, mut ms) = (0u32, 0f64, 0f64);
@@ -285,38 +302,25 @@ impl FixedRule for ShortestPathDijkstraGpu {
         let undirected = payload.bool_option("undirected", Some(false))?;
 
         let el = edges.as_edge_list(undirected, true)?;
-        let mut starting_nodes = BTreeSet::new();
-        for tuple in starting.iter()? {
-            if let Some(idx) = el.inv_indices.get(&tuple?[0]) {
-                starting_nodes.insert(*idx);
-            }
-        }
+        let starting_nodes: BTreeSet<u32> = el.lookup_first_fields(&starting)?.into_iter().collect();
         let termination_nodes = match termination {
             Err(_) => None,
-            Ok(t) => {
-                let mut tn = BTreeSet::new();
-                for tuple in t.iter()? {
-                    if let Some(idx) = el.inv_indices.get(&tuple?[0]) {
-                        tn.insert(*idx);
-                    }
-                }
-                Some(tn)
-            }
+            Ok(t) => Some(el.lookup_first_fields(&t)?.into_iter().collect::<BTreeSet<u32>>()),
         };
         if starting_nodes.is_empty() || el.indices.is_empty() {
             return Ok(());
         }
         let n = el.indices.len();
         let sources: Vec<u32> = starting_nodes.iter().copied().collect();
-        let g = DevGraph::stage(&el)?;
+        let g = &el.g;
         let pm = PoisonMirror::new(poison.clone());
         let ties = keep_ties && termination_nodes.is_some();
         let mut in_edges: Vec<Vec<(u32, f32)>> = vec![];
         if ties {
             in_edges.resize(n, vec![]);
-            let w = el.w.as_ref().unwrap();
-            for e in 0..el.src.len() {
-                in_edges[el.dst[e] as usize].push((el.src[e], w[e]));
+            let (src, dst, w) = el.edges()?;
+            for e in 0..src.len() {
+                in_edges[dst[e] as usize].push((src[e], w[e]));
             }
         }
         let mut dist = vec![0f32; sources.len() * n];
@@ -393,7 +397,7 @@ macro_rules! centrality_rule {
                 if el.indices.is_empty() {
                     return Ok(());
                 }
-                let g = DevGraph::stage(&el)?;
+                let g = &el.g;
                 let pm = PoisonMirror::new(poison);
                 let mut res = vec![0f32; el.indices.len()];
                 let mut ms = 0f64;
@@ -426,7 +430,7 @@ impl FixedRule for ClusteringCoefficientsGpu {
             return Ok(());
         }
         let n = el.indices.len();
-        let g = DevGraph::stage(&el)?;
+        let g = &el.g;
         let pm = PoisonMirror::new(poison);
         let (mut cc, mut tri, mut deg) = (vec![0f64; n], vec![0u64; n], vec![0u64; n]);
         let mut ms = 0f64;
@@ -519,17 +523,9 @@ impl FixedRule for KShortestPathYenGpu {
         let undirected = payload.bool_option("undirected", Some(false))?; // yen.rs:38
         let k = payload.pos_integer_option("k", None)?; // yen.rs:39
         let el = edges.as_edge_list(undirected, true)?;
-        let (mut starts, mut goals_set) = (BTreeSet::new(), BTreeSet::new()); // yen.rs:43-58
-        for t in starting.iter()? {
-            if let Some(i) = el.inv_indices.get(&t?[0]) {
-                starts.insert(*i);
-            }
-        }
-        for t in termination.iter()? {
-            if let Some(i) = el.inv_indices.get(&t?[0]) {
-                goals_set.insert(*i);
-            }
-        }
+        // yen.rs:43-58
+        let starts: BTreeSet<u32> = el.lookup_first_fields(&starting)?.into_iter().collect();
+        let goals_set: BTreeSet<u32> = el.lookup_first_fields(&termination)?.into_iter().collect();
         struct Pair {
             start: u32,
             k_shortest: Vec<(f32, Vec<u32>)>,
@@ -546,13 +542,14 @@ impl FixedRule for KShortestPathYenGpu {
         if ps.is_empty() {
             return Ok(());
         }
-        // the first edge s->d in adjacency order supplies the root-path cost (yen.rs:171-183)
+        // the first edge s->d in adjacency order supplies the root-path cost (yen.rs:171-183); the CSR
+        // keeps parallel edges in input order
         let mut first_edge: BTreeMap<(u32, u32), f32> = BTreeMap::new();
-        let w = el.w.as_ref().unwrap();
-        for e in 0..el.src.len() {
-            first_edge.entry((el.src[e], el.dst[e])).or_insert(w[e]);
+        let (src, dst, w) = el.edges()?;
+        for e in 0..src.len() {
+            first_edge.entry((src[e], dst[e])).or_insert(w[e]);
         }
-        let g = DevGraph::stage(&el)?;
+        let g = &el.g;
         let pm = PoisonMirror::new(poison.clone());
         let batch: Vec<YenSearch> = (0..ps.len())
             .map(|pi| YenSearch { pair: pi, i: usize::MAX, from: ps[pi].start, forb_nodes: vec![], forb_edges: vec![] })
