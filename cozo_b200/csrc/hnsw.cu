@@ -42,8 +42,9 @@ struct SearchParams {
 
 
 // hnsw_knn's tail (hnsw.rs:943-956, 997-1006) for the query of this warp: walk the beam nearest first, drop
-// `dist > radius` and rows the filter rejects, keep the first k, pad the rest.  Without a filter the kept
-// entries are a prefix of the sorted array.  Returns the number of results.
+// `dist > radius` and rows the filter rejects, keep the first k, pad the rest.  Without a filter the beam is cut to k
+// before the radius test, and without either the kept entries are a prefix of the sorted array.  A radius does not
+// keep a prefix: NaN keys sort last and pass it (`NaN > r` is false).  Returns the number of results.
 __device__ __forceinline__ uint32_t emit_results(const SearchParams& p, const WarpCtx& w, uint32_t qi, int lane,
                                                  bool searched) {
   auto store = [&](uint32_t i, uint32_t oid, float od) {
@@ -58,28 +59,20 @@ __device__ __forceinline__ uint32_t emit_results(const SearchParams& p, const Wa
     }
   };
   uint32_t found = 0;
-  if (searched && !p.filter_mask) {
+  if (searched && !p.filter_mask && !p.has_radius) {
     found = w.len < p.k ? w.len : p.k;
-    if (p.has_radius) {
-      uint32_t c = 0;
-      for (uint32_t base_i = 0; base_i < found; base_i += 32) {
-        uint32_t i = base_i + lane;
-        bool in = i < found && !((double)w.fd[i] > p.radius);
-        c += __popc(__ballot_sync(0xffffffffu, in));
-      }
-      found = c;
-    }
     for (uint32_t i = lane; i < found; i += 32) store(i, w.fi[i] & IDMASK, w.fd[i]);
   } else if (searched) {
-    for (uint32_t base_i = 0; base_i < w.len && found < p.k; base_i += 32) {
+    const uint32_t lim = p.filter_mask || w.len < p.k ? w.len : p.k;
+    for (uint32_t base_i = 0; base_i < lim && found < p.k; base_i += 32) {
       const uint32_t i = base_i + lane;
-      bool ok = i < w.len;
+      bool ok = i < lim;
       uint32_t id = 0;
       float d = 0.f;
       if (ok) {
         id = w.fi[i] & IDMASK;
         d = w.fd[i];
-        ok = ((p.filter_mask[id >> 5] >> (id & 31)) & 1u) && !(p.has_radius && (double)d > p.radius);
+        ok = (!p.filter_mask || ((p.filter_mask[id >> 5] >> (id & 31)) & 1u)) && !(p.has_radius && (double)d > p.radius);
       }
       const uint32_t bal = __ballot_sync(0xffffffffu, ok);
       const uint32_t pos = found + __popc(bal & ((1u << lane) - 1));

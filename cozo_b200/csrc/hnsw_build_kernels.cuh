@@ -217,7 +217,8 @@ __device__ __forceinline__ uint32_t heuristic_select(const HnswDev& g, const flo
 // (the reference pays the same), so the builder restricts it to small batches.  The base vector's own key is skipped:
 // the reference's shrink path would admit it (and overwrite its self-loop row, hnsw.rs:413-432), which the oracle
 // treats as a defect too.
-__device__ __forceinline__ uint32_t f32_order_key(float f) {
+__device__ __forceinline__ uint32_t f32_order_key(float f) {  // every NaN (either sign) after +inf, as OrderedFloat
+  if (f != f) return 0xFFFFFFFFu;
   const uint32_t b = __float_as_uint(f);
   return b ^ ((b >> 31) ? 0xFFFFFFFFu : 0x80000000u);
 }
@@ -472,12 +473,12 @@ __device__ __forceinline__ void build_link_body(const HnswDev& g, const BuildDev
       u_d[deg + lane] = ad;
     }
     __syncwarp();
-    for (uint32_t j = lane; j < nc; j += 32) {  // rank sort by (distance, position)
+    for (uint32_t j = lane; j < nc; j += 32) {  // rank sort by (distance, position); NaN after every number (OrderedFloat)
       float dj = u_d[j];
       uint32_t rank = 0;
       for (uint32_t x = 0; x < nc; ++x) {
         float dx = u_d[x];
-        rank += (dx < dj) || (dx == dj && x < j);
+        rank += dj != dj ? (dx == dx || x < j) : (dx < dj || (dx == dj && x < j));
       }
       s_id[rank] = u_id[j];
       s_d[rank] = dj;

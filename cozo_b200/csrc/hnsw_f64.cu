@@ -63,12 +63,13 @@ __device__ __forceinline__ double dist64(const double* q, const double* __restri
   return 1.0 - a / sqrt(qnorm * b);
 }
 
-// found_nn.push + pop-if-over-ef (hnsw.rs:577-580) on the sorted array; equal keys keep arrival order
+// found_nn.push + pop-if-over-ef (hnsw.rs:577-580) on the sorted array; equal keys keep arrival order, NaN sorts after
+// every number and equal to NaN (OrderedFloat), as in sorted_insert
 __device__ __forceinline__ void sorted_insert64(WarpCtx& w, double* fd, uint32_t ef, double d, uint32_t id, int lane) {
   uint32_t pos = 0;
   for (uint32_t base = 0; base < w.len; base += 32) {
     uint32_t i = base + lane;
-    bool le = (i < w.len) && (fd[i] <= d);
+    bool le = (i < w.len) && (fd[i] <= d || d != d);
     uint32_t bal = __ballot_sync(0xffffffffu, le);
     pos += __popc(bal);
     if (bal != 0xffffffffu) break;
@@ -210,10 +211,12 @@ __global__ void __launch_bounds__(128) hnsw_search_f64_kernel(HnswDev g, Search6
       __syncwarp();
       for (uint32_t lvl = g.top_level; lvl >= 1; --lvl) search_level64<METRIC>(g, p, w, fd, q, qn, 1, lvl, lane);
       search_level64<METRIC>(g, p, w, fd, q, qn, p.ef, 0, lane);
-      // hnsw.rs:943-956, 997-1006: radius, filter verdicts, then the first k
-      for (uint32_t base_i = 0; base_i < w.len && found < p.k; base_i += 32) {
+      // hnsw.rs:943-956, 997-1006: radius, filter verdicts, then the first k; without a filter the beam is cut to k
+      // before the radius test (NaN keys sort last and pass it)
+      const uint32_t lim = p.filter_mask || w.len < p.k ? w.len : p.k;
+      for (uint32_t base_i = 0; base_i < lim && found < p.k; base_i += 32) {
         const uint32_t i = base_i + lane;
-        bool ok = i < w.len;
+        bool ok = i < lim;
         uint32_t id = 0;
         double d2 = 0.0;
         if (ok) {

@@ -139,9 +139,20 @@ static double vec_dist64(int metric, const double* a, const double* b, size_t n)
 // pop/peek = max priority.  Order among EQUAL priorities is unspecified in the
 // crate (heap-shape dependent); here it is made deterministic: larger id wins
 // in a max-queue.  Tests therefore use tie-free data (SURVEY.md §7 hard parts).
+// Priorities compare as OrderedFloat<f64>: NaN is greater than every number
+// (+inf included) and equal to NaN, so a NaN key is an ordinary priority.
 // ---------------------------------------------------------------------------
+struct OrderedLess {
+  bool operator()(const std::pair<double, uint32_t>& a, const std::pair<double, uint32_t>& b) const {
+    const bool an = std::isnan(a.first), bn = std::isnan(b.first);
+    if (an != bn) return bn;
+    if (!an && a.first != b.first) return a.first < b.first;
+    return a.second < b.second;
+  }
+};
+using PQSet = std::set<std::pair<double, uint32_t>, OrderedLess>;
 struct MaxPQ {
-  std::set<std::pair<double, uint32_t>> s;
+  PQSet s;
   std::map<uint32_t, double> pr;
   size_t size() const { return s.size(); }
   bool empty() const { return s.empty(); }
@@ -170,7 +181,7 @@ struct MaxPQ {
 };
 // Min-queue = PriorityQueue<_, Reverse<OrderedFloat>>; smaller id wins ties.
 struct MinPQ {
-  std::set<std::pair<double, uint32_t>> s;
+  PQSet s;
   std::map<uint32_t, double> pr;
   size_t size() const { return s.size(); }
   bool empty() const { return s.empty(); }
