@@ -23,7 +23,7 @@ E_INVAL, E_CUDA, E_NODEV, E_NOMEM, E_KILLED, E_UNSUP = -1, -2, -3, -4, -5, -6
 EXPORTS = [
     "cozo_gpu_init", "cozo_gpu_shutdown", "cozo_gpu_last_error", "cozo_gpu_device_count", "cozo_gpu_set_option",
     "cozo_gpu_get_option", "cozo_gpu_hnsw_stage", "cozo_gpu_hnsw_free", "cozo_gpu_hnsw_search",
-    "cozo_gpu_hnsw_search_dev", "cozo_gpu_hnsw_search_scatter_dev", "cozo_gpu_hnsw_build", "cozo_gpu_hnsw_insert", "cozo_gpu_hnsw_insert_at", "cozo_gpu_hnsw_remove", "cozo_gpu_hnsw_update", "cozo_gpu_hnsw_info", "cozo_gpu_hnsw_level_size",
+    "cozo_gpu_hnsw_search_dev", "cozo_gpu_hnsw_search_scatter_dev", "cozo_gpu_hnsw_build", "cozo_gpu_hnsw_insert", "cozo_gpu_hnsw_insert_at", "cozo_gpu_hnsw_remove", "cozo_gpu_hnsw_compact", "cozo_gpu_hnsw_update", "cozo_gpu_hnsw_info", "cozo_gpu_hnsw_level_size",
     "cozo_gpu_hnsw_export_level", "cozo_gpu_hnsw_export_level_dist", "cozo_gpu_hnsw_export_live", "cozo_gpu_hnsw_vectors_dev", "cozo_gpu_topk_merge_dev", "cozo_gpu_graph_stage",
     "cozo_gpu_graph_free", "cozo_gpu_graph_export", "cozo_gpu_pagerank", "cozo_gpu_sssp_multi", "cozo_gpu_closeness",
     "cozo_gpu_betweenness", "cozo_gpu_clustering", "cozo_gpu_sssp_paths",
@@ -91,6 +91,7 @@ def load():
     L.cozo_gpu_hnsw_insert.argtypes = [vp, vp, u32, C.c_int32, u32, C.c_int32, vp]
     L.cozo_gpu_hnsw_insert_at.argtypes = [vp, vp, vp, u32, C.c_int32, u32, C.c_int32, vp]
     L.cozo_gpu_hnsw_remove.argtypes = [vp, vp, u32]
+    L.cozo_gpu_hnsw_compact.argtypes = [vp, vp]
     L.cozo_gpu_hnsw_update.argtypes = [vp, vp, vp, u32, u32, C.c_int32]
     L.cozo_gpu_hnsw_info.argtypes = [vp, vp, vp, vp, vp]
     L.cozo_gpu_hnsw_level_size.argtypes = [vp, u32, vp, vp]
@@ -270,6 +271,12 @@ class HnswIndex:
     def remove(self, ids):
         ids = np.ascontiguousarray(ids, np.uint32)
         _check(load().cozo_gpu_hnsw_remove(self._h, _p(ids), ids.size))
+
+    def compact(self) -> np.ndarray:
+        """drop every removed id; live ids move down in key order.  Returns old_to_new (NONE for a removed id)."""
+        out = np.zeros(self.info()[0], np.uint32)
+        _check(load().cozo_gpu_hnsw_compact(self._h, _p(out)))
+        return out
 
     def info(self):
         n, dim, nl, ep = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32()

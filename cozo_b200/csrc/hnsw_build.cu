@@ -19,6 +19,7 @@
 // per arrival.  Soft-deleted (`ignore_link`) rows are not materialised: the
 // staged layout only holds what hnsw_get_neighbours would return.
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <cmath>
@@ -792,6 +793,171 @@ extern "C" int cozo_gpu_hnsw_insert_at(cozo_gpu_hnsw_t* h, const uint32_t* posit
   rc = hnsw_insert_ids(h, new_ids, 0, true);
   if (rc) return rc;
   if (out_ids) std::copy(new_ids.begin(), new_ids.end(), out_ids);
+  return 0;
+}
+
+// Moves rows [first, n) of one array (row_bytes each) to rows map[j], dropping rows that map to NONE, `chunk` rows at a
+// time from the head through `stage`.  Destinations are never above their sources, so a chunk only overwrites rows
+// already read, and no second copy of the array is needed.  On the legacy default stream.
+static int compact_rows(void* base, size_t row_bytes, uint32_t first, uint32_t n, uint8_t* stage, uint64_t chunk,
+                        const uint32_t* d_map) {
+  uint8_t* p = static_cast<uint8_t*>(base);
+  for (uint32_t lo = first; lo < n;) {
+    const uint32_t rows = (uint32_t)std::min<uint64_t>(chunk, n - lo);
+    H_CUDA(cudaMemcpyAsync(stage, p + (size_t)lo * row_bytes, (size_t)rows * row_bytes, cudaMemcpyDeviceToDevice, 0));
+    if (row_bytes % 16 == 0) {
+      const uint32_t e = (uint32_t)(row_bytes / 16);
+      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
+      compact_rows_kernel<uint4><<<(uint32_t)((threads + 255) / 256), 256>>>(
+          reinterpret_cast<const uint4*>(stage), reinterpret_cast<uint4*>(p), e, lo, rows, d_map);
+    } else if (row_bytes % 4 == 0) {
+      const uint32_t e = (uint32_t)(row_bytes / 4);
+      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
+      compact_rows_kernel<uint32_t><<<(uint32_t)((threads + 255) / 256), 256>>>(
+          reinterpret_cast<const uint32_t*>(stage), reinterpret_cast<uint32_t*>(p), e, lo, rows, d_map);
+    } else {
+      const uint32_t e = (uint32_t)row_bytes;
+      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
+      compact_rows_kernel<uint8_t><<<(uint32_t)((threads + 255) / 256), 256>>>(stage, p, e, lo, rows, d_map);
+    }
+    H_CUDA(cudaGetLastError());
+    lo += rows;
+  }
+  return 0;
+}
+
+static int compact_ids(uint32_t* ids, size_t count, const uint32_t* d_map, uint32_t* d_bad) {
+  if (!count) return 0;
+  compact_ids_kernel<<<(uint32_t)((count + 255) / 256), 256>>>(ids, count, d_map, d_bad);
+  H_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Drops every removed id.  Live id j becomes j - #{removed ids < j}; the upper-layer rows of removed ids go too.  The
+// map is monotone, so stored neighbour order, edge distances and the entry rule are unchanged.  Capacity is kept.
+extern "C" int cozo_gpu_hnsw_compact(cozo_gpu_hnsw_t* h, uint32_t* old_to_new) {
+  if (!h) return set_error(COZO_GPU_EINVAL, "null index handle");
+  int rc = ensure_init();
+  if (rc) return rc;
+  if (h->f64) return set_error(COZO_GPU_EUNSUP, "F64 indexes are search-only on the device: re-stage after a mutation");
+  HnswDev& g = h->dev;
+  const uint32_t n0 = g.n;
+  std::vector<uint32_t> map(n0);
+  uint32_t n1 = 0, first = n0;
+  for (uint32_t j = 0; j < n0; ++j) {
+    const bool keep = j >= h->live.size() || h->live[j];
+    map[j] = keep ? n1++ : NONE;
+    if (!keep && first == n0) first = j;
+  }
+  if (n1 == n0) {  // nothing removed: nothing moves
+    if (old_to_new) std::copy(map.begin(), map.end(), old_to_new);
+    return 0;
+  }
+  // removed ids exist only after cozo_gpu_hnsw_remove, which made the build state (degrees, distances, owners)
+  // an asynchronous search_dev may still be reading the rows about to move
+  H_CUDA(cudaDeviceSynchronize());
+  const uint32_t up0 = (uint32_t)h->up_rows;
+
+  // scratch first, so that running out of memory leaves the index as it was
+  struct Scratch {
+    uint32_t *map = nullptr, *keep = nullptr, *up_map = nullptr, *counters = nullptr;
+    uint8_t* stage = nullptr;
+    void* cub_tmp = nullptr;
+    ~Scratch() {
+      void* ptrs[] = {map, keep, up_map, counters, stage, cub_tmp};
+      for (void* p : ptrs)
+        if (p) cudaFree(p);
+    }
+  } sc;
+  H_CUDA(cudaMalloc(&sc.map, (size_t)n0 * 4));
+  H_CUDA(cudaMalloc(&sc.keep, ((size_t)up0 + 1) * 4));
+  H_CUDA(cudaMalloc(&sc.up_map, ((size_t)up0 + 1) * 4));
+  H_CUDA(cudaMalloc(&sc.counters, 8));
+  size_t cub_bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, sc.keep, sc.up_map, (int)(up0 + 1));
+  H_CUDA(cudaMalloc(&sc.cub_tmp, std::max<size_t>(cub_bytes, 16)));
+  H_CUDA(cudaMemcpy(sc.map, map.data(), (size_t)n0 * 4, cudaMemcpyHostToDevice));
+  // counters[0]: first dropped upper row (NONE: none), counters[1]: stored ids that name a removed id
+  H_CUDA(cudaMemset(sc.counters, 0xFF, 4));
+  H_CUDA(cudaMemset(sc.counters + 1, 0, 4));
+  // the upper-row map: rows whose owner stays, in row order
+  upper_keep_kernel<<<(up0 + 256) / 256, 256>>>(h->d_up_owner, up0, sc.map, sc.keep);
+  H_CUDA(cudaGetLastError());
+  cub::DeviceScan::ExclusiveSum(sc.cub_tmp, cub_bytes, sc.keep, sc.up_map, (int)(up0 + 1));
+  if (up0) upper_map_kernel<<<(up0 + 255) / 256, 256>>>(sc.keep, up0, sc.up_map, sc.counters);
+  H_CUDA(cudaGetLastError());
+  uint32_t up1 = 0, up_first = NONE;
+  H_CUDA(cudaMemcpy(&up1, sc.up_map + up0, 4, cudaMemcpyDeviceToHost));
+  H_CUDA(cudaMemcpy(&up_first, sc.counters, 4, cudaMemcpyDeviceToHost));
+  if (up_first == NONE) up_first = up0;
+
+  // Per-node and upper-row arrays with their row sizes (code rows only where the index has them).  Each array moves
+  // through the staging buffer in chunks of kStageBytes / row_bytes rows, or of `hnsw.shift_chunk_rows` rows when that
+  // is set.
+  const size_t kStageBytes = (size_t)64 << 20;
+  const size_t vec_row = (size_t)g.ld * 4, adj_row = (size_t)g.s0 * 4, up_row = (size_t)g.su * 4;
+  const size_t row_bytes[] = {vec_row, g.code_ld, adj_row, adj_row, 4, 4, 1, 1, up_row, up_row, 4, 4};
+  constexpr size_t kNodeArrays = 8, kArrays = 12;
+  const int64_t chunk_opt = get_option("hnsw.shift_chunk_rows", 0);
+  auto chunk_rows = [&](size_t a) {
+    const uint64_t moving = a < kNodeArrays ? n0 - first : up0 - up_first;
+    const uint64_t c = chunk_opt > 0 ? (uint64_t)chunk_opt : std::max<uint64_t>(1, kStageBytes / row_bytes[a]);
+    return std::max<uint64_t>(1, std::min(c, moving));
+  };
+  size_t stage_bytes = 1;
+  for (size_t a = 0; a < kArrays; ++a) stage_bytes = std::max(stage_bytes, (size_t)chunk_rows(a) * row_bytes[a]);
+  H_CUDA(cudaMalloc(&sc.stage, stage_bytes));
+
+  if (!h->vec_owned) {  // never write into a borrowed buffer
+    rc = hnsw_reserve(h, h->borrowed_rows + 1, h->up_rows);
+    if (rc) return rc;
+  }
+  // after the private copy: the arrays' current addresses
+  void* const moved[] = {h->d_vec, g.codes ? h->d_codes : nullptr, h->d_adj0, h->d_adj0_dist, h->d_deg0,
+                         h->d_upper_off, h->d_node_level, h->d_dead, h->d_adj_up, h->d_adj_up_dist, h->d_deg_up,
+                         h->d_up_owner};
+  // 1. every array: kept rows move down, rows before the first dropped one stay
+  for (size_t a = 0; a < kArrays; ++a) {
+    if (!moved[a]) continue;
+    rc = a < kNodeArrays ? compact_rows(moved[a], row_bytes[a], first, n0, sc.stage, chunk_rows(a), sc.map)
+                         : compact_rows(moved[a], row_bytes[a], up_first, up0, sc.stage, chunk_rows(a), sc.up_map);
+    if (rc) return rc;
+  }
+  // 2. every stored id of a kept row: node ids through the node map, upper_off through the row map
+  rc = compact_ids(h->d_adj0, (size_t)n1 * g.s0, sc.map, sc.counters + 1);
+  if (!rc) rc = compact_ids(h->d_adj_up, (size_t)up1 * g.su, sc.map, sc.counters + 1);
+  if (!rc) rc = compact_ids(h->d_up_owner, up1, sc.map, sc.counters + 1);
+  if (!rc) rc = compact_ids(h->d_upper_off, n1, sc.up_map, sc.counters + 1);
+  if (rc) return rc;
+  // 3. the freed rows go back to the state of unused capacity, which append_nodes expects
+  H_CUDA(cudaMemsetAsync(h->d_vec + (size_t)n1 * g.ld, 0, (size_t)(n0 - n1) * vec_row, 0));
+  H_CUDA(cudaMemsetAsync(h->d_adj0 + (size_t)n1 * g.s0, 0xFF, (size_t)(n0 - n1) * adj_row, 0));
+  H_CUDA(cudaMemsetAsync(h->d_adj0_dist + (size_t)n1 * g.s0, 0, (size_t)(n0 - n1) * adj_row, 0));
+  H_CUDA(cudaMemsetAsync(h->d_deg0 + n1, 0, (size_t)(n0 - n1) * 4, 0));
+  H_CUDA(cudaMemsetAsync(h->d_upper_off + n1, 0xFF, (size_t)(n0 - n1) * 4, 0));
+  H_CUDA(cudaMemsetAsync(h->d_node_level + n1, 0, n0 - n1, 0));
+  H_CUDA(cudaMemsetAsync(h->d_dead + n1, 0, n0 - n1, 0));
+  if (up1 < up0) {
+    H_CUDA(cudaMemsetAsync(h->d_adj_up + (size_t)up1 * g.su, 0xFF, (size_t)(up0 - up1) * up_row, 0));
+    H_CUDA(cudaMemsetAsync(h->d_adj_up_dist + (size_t)up1 * g.su, 0, (size_t)(up0 - up1) * up_row, 0));
+    H_CUDA(cudaMemsetAsync(h->d_deg_up + up1, 0, (size_t)(up0 - up1) * 4, 0));
+    H_CUDA(cudaMemsetAsync(h->d_up_owner + up1, 0xFF, (size_t)(up0 - up1) * 4, 0));
+  }
+  uint32_t bad = 0;
+  H_CUDA(cudaMemcpy(&bad, sc.counters + 1, 4, cudaMemcpyDeviceToHost));
+  if (bad) return set_error(COZO_GPU_ECUDA, "internal: %u stored ids name removed ids", bad);
+
+  // host copies
+  std::vector<uint8_t> level(n1);
+  for (uint32_t j = 0; j < n0; ++j)
+    if (map[j] != NONE) level[map[j]] = h->node_level[j];
+  h->node_level.swap(level);
+  h->live.assign(n1, 1);
+  h->n_live = n1;
+  if (g.entry != NONE) g.entry = map[g.entry];
+  h->up_rows = up1;
+  g.n = n1;
+  if (old_to_new) std::copy(map.begin(), map.end(), old_to_new);
   return 0;
 }
 

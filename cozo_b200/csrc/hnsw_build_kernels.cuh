@@ -634,4 +634,50 @@ __global__ void place_new_rows_kernel(const uint32_t* new_ids, uint32_t count, c
   }
 }
 
+// ---- drop removed ids (cozo_gpu_hnsw_compact) -------------------------------------------------------------------
+// map: old row -> new row, NONE for a dropped row; monotone, never above the old row.
+
+// Forward twin of shift_rows_kernel: rows j0 .. j0+rows-1, staged in `src`, are written to rows map[j] of `dst`;
+// dropped rows are not written.
+template <class T>
+__global__ void __launch_bounds__(256) compact_rows_kernel(const T* src, T* dst, uint32_t row_elems, uint32_t j0,
+                                                           uint32_t rows, const uint32_t* map) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool per_warp = row_elems >= 32;
+  const size_t r = per_warp ? t >> 5 : t;
+  if (r >= rows) return;
+  const uint32_t to = map[j0 + r];
+  if (to == NONE) return;
+  for (uint32_t c = per_warp ? (uint32_t)(t & 31) : 0; c < row_elems; c += per_warp ? 32 : 1)
+    dst[(size_t)to * row_elems + c] = src[(size_t)r * row_elems + c];
+}
+
+// every stored id of a kept row through `map`; NONE stays NONE.  An id that maps to NONE names a dropped row that a
+// kept row still points at: counted in *bad (hnsw_remove leaves none).
+__global__ void compact_ids_kernel(uint32_t* ids, size_t count, const uint32_t* map, uint32_t* bad) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  const uint32_t v = ids[i];
+  if (v == NONE) return;
+  const uint32_t to = map[v];
+  if (to == NONE) atomicAdd(bad, 1u);
+  ids[i] = to;
+}
+
+// keep[r] = 1 for the upper-layer rows whose owner stays; keep[up_rows] = 0 makes the exclusive sum's last element
+// the number of kept rows
+__global__ void upper_keep_kernel(const uint32_t* owner, uint32_t up_rows, const uint32_t* map, uint32_t* keep) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r <= up_rows) keep[r] = r < up_rows && map[owner[r]] != NONE;
+}
+
+// the exclusive sum of keep[] -> the row map: NONE for dropped rows.  The one dropped row whose sum equals its own
+// row number is the first dropped row (every row before it is kept): written to *first_drop.
+__global__ void upper_map_kernel(const uint32_t* keep, uint32_t up_rows, uint32_t* map, uint32_t* first_drop) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= up_rows || keep[r]) return;
+  if (map[r] == r) *first_drop = r;
+  map[r] = NONE;
+}
+
 }  // namespace cozo

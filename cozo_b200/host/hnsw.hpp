@@ -720,6 +720,25 @@ struct StagedHnswIndex {
     n_removed += ids.size();
   }
 
+  // cozo_gpu_hnsw_compact: the removed ids leave the device copy and their keys leave the dictionary, so that dense ids
+  // are again the key ranks of the indexed rows, as a fresh stage gives them
+  void compact() {
+    sync_dictionary();
+    if (keys.empty()) return;
+    std::vector<uint32_t> old_to_new(keys.size());
+    gpu_check(cozo_gpu_hnsw_compact(h, old_to_new.data()));
+    std::vector<CompoundKey> k2;
+    for (size_t i = 0; i < keys.size(); ++i)
+      if (old_to_new[i] != COZO_GPU_NONE) {
+        if (old_to_new[i] != k2.size()) throw CozoError("", "device ids out of step with the key dictionary");
+        k2.push_back(std::move(keys[i]));
+      }
+    keys.swap(k2);
+    live.assign(keys.size(), 1);
+    key_ids.clear();
+    for (uint32_t i = 0; i < keys.size(); ++i) key_ids.emplace(keys[i], i);
+  }
+
   // SessionTx::hnsw_put (hnsw.rs:679-727) for a batch of rows, then the rows go into the base relation.
   // `filter` is the index_filter predicate (rows failing it are un-indexed, hnsw.rs:688-693).
   void put_rows(RelationHandle& base, const std::vector<Tuple>& all_rows,

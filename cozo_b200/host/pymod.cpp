@@ -172,6 +172,7 @@ struct PyHnswIndex {
     ix.put_rows(base.rel, to_rows(rows), f);
   }
   void remove_rows(PyRelation& base, py::handle rows) { ix.remove_rows(base.rel, to_rows(rows)); }
+  void compact() { ix.compact(); }
   py::list to_index_rows(const PyRelation& base) const { return from_rows(ix.to_index_rows(base.rel)); }
   py::dict info() const {
     py::dict d;
@@ -280,6 +281,7 @@ PYBIND11_MODULE(_cozo_host, m) {
       .def("build", &PyHnswIndex::build)
       .def("put_rows", &PyHnswIndex::put_rows, py::arg("base"), py::arg("rows"), py::arg("filter") = py::none())
       .def("remove_rows", &PyHnswIndex::remove_rows)
+      .def("compact", &PyHnswIndex::compact)
       .def("to_index_rows", &PyHnswIndex::to_index_rows)
       .def("info", &PyHnswIndex::info)
       .def_property(

@@ -21,7 +21,7 @@
  *     a workspace from a bounded pool.  Graph algorithm calls are thread-safe per
  *     handle too (the staged graph is read-only, every call owns its buffers) but
  *     run on the default stream, i.e. concurrent calls serialise on the device.
- *     stage / free / build / insert / insert_at / update / remove are not concurrent with
+ *     stage / free / build / insert / insert_at / update / remove / compact are not concurrent with
  *     any other call on the same handle.
  *   - `poison` parameters point at a 32-bit flag mirroring the AtomicBool inside
  *     Poison (runtime/db.rs:1926-1942; INTEGRATION.md shows the mirror); it is
@@ -212,6 +212,17 @@ int cozo_gpu_hnsw_insert_at(cozo_gpu_hnsw_t* h, const uint32_t* positions, const
                             int32_t vectors_on_device, uint32_t ef_construction,
                             int32_t keep_pruned_connections, uint32_t* out_ids);
 int cozo_gpu_hnsw_remove(cozo_gpu_hnsw_t* h, const uint32_t* ids, uint32_t count);
+/* Drop every removed id (cozo_gpu_hnsw_remove, or un-indexed by the host) from the handle.
+ * Live id j becomes j - #{removed ids < j}, so dense ids stay in key order.
+ * old_to_new [n before the call] (nullable): new id, or COZO_GPU_NONE for a removed id.
+ * The map is monotone: stored neighbour order, edge distances, the entry-point rule, the top layer
+ * and the level law's state are unchanged; the upper-layer rows of removed ids go too.  Allocated
+ * capacity is kept for later inserts.  With no removed id nothing moves; with every id removed the
+ * index is empty (n = 0, entry COZO_GPU_NONE), as if staged from the canary row alone.  Waits for
+ * device work already enqueued on the handle (an asynchronous search_dev) before moving rows.
+ * COZO_GPU_EUNSUP for an F64 index; all scratch is allocated before any row moves, so
+ * COZO_GPU_ENOMEM leaves the handle as it was.  A borrowed vector buffer is never written. */
+int cozo_gpu_hnsw_compact(cozo_gpu_hnsw_t* h, uint32_t* old_to_new);
 /* hnsw_put of a changed vector under an existing key (hnsw.rs:175-182: remove, then insert again);
  * vectors [count x dim] host memory, ids distinct.  The node keeps its id and layer.  Removed ids
  * may be revived this way. */

@@ -91,6 +91,7 @@ extern "C" {
     pub fn cozo_gpu_hnsw_insert(h: *mut CozoGpuHnsw, vectors: *const f32, count: u32, vectors_on_device: i32, ef_construction: u32, keep_pruned_connections: i32, first_id: *mut u32) -> c_int;
     pub fn cozo_gpu_hnsw_insert_at(h: *mut CozoGpuHnsw, positions: *const u32, vectors: *const f32, count: u32, vectors_on_device: i32, ef_construction: u32, keep_pruned_connections: i32, out_ids: *mut u32) -> c_int;
     pub fn cozo_gpu_hnsw_remove(h: *mut CozoGpuHnsw, ids: *const u32, count: u32) -> c_int;
+    pub fn cozo_gpu_hnsw_compact(h: *mut CozoGpuHnsw, old_to_new: *mut u32) -> c_int;
     pub fn cozo_gpu_hnsw_update(h: *mut CozoGpuHnsw, ids: *const u32, vectors: *const f32, count: u32, ef_construction: u32, keep_pruned_connections: i32) -> c_int;
     pub fn cozo_gpu_hnsw_info(h: *mut CozoGpuHnsw, n_vectors: *mut u32, dim: *mut u32, n_levels: *mut u32, entry_point: *mut u32) -> c_int;
     pub fn cozo_gpu_hnsw_level_size(h: *mut CozoGpuHnsw, level: u32, n_nodes: *mut u32, n_edges: *mut u64) -> c_int;

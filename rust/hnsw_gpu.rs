@@ -58,9 +58,9 @@ pub(crate) struct StagedIndex {
 ///   hnsw_remove <- query/stored.rs:995-997
 ///   index drop  <- runtime/relation.rs:1383 (`hnsw_indices.remove`)
 /// each calls `gpu_index_invalidate(idx_handle.id)` before touching the relation, except that a `:put` whose
-/// compound keys are all new goes through `gpu_index_put_new_keys` instead.  The next search re-stages a dropped
-/// copy (changed vectors and removals can likewise go to cozo_gpu_hnsw_update / _remove —
-/// `StagedHnswIndex::put_rows` / `remove_rows` in the C++ twin show the exact rules).
+/// compound keys are all new goes through `gpu_index_put_new_keys`, and `:rm` through `gpu_index_remove_keys`,
+/// instead.  The next search re-stages a dropped copy (changed vectors can likewise go to cozo_gpu_hnsw_update —
+/// `StagedHnswIndex::put_rows` in the C++ twin shows the exact rules).
 /// A staged copy is only handed to readers whose transaction started after the staging.
 pub(crate) fn gpu_index_invalidate(idx_rel_id: crate::runtime::relation::RelationId) {
     STAGED.lock().unwrap().remove(&idx_rel_id.0);
@@ -100,6 +100,44 @@ pub(crate) fn gpu_index_put_new_keys(
     for (i, (k, _)) in new.iter().enumerate() {
         staged.keys.insert(ids[i] as usize, k.clone()); // ids ascend: key i lands after keys 0..i
     }
+    Ok(())
+}
+
+/// hnsw_remove of whole tuples (query/stored.rs:995-997 -> hnsw.rs:728-753), absorbed in place: every compound key
+/// of each removed tuple key goes to cozo_gpu_hnsw_remove, then cozo_gpu_hnsw_compact drops the removed ids, so the
+/// copy stays in the id space a fresh staging of the relation gives (dense id = key rank of the remaining rows).
+/// F64 copies, copies still shared with a reader, and any error drop the copy instead: the next search re-stages it.
+pub(crate) fn gpu_index_remove_keys(idx_rel_id: crate::runtime::relation::RelationId, tuple_keys: &[Tuple]) -> Result<()> {
+    let mut map = STAGED.lock().unwrap();
+    let Some(arc) = map.get_mut(&idx_rel_id.0) else { return Ok(()) };
+    let staged = match Arc::get_mut(arc) {
+        Some(s) if !s.f64_index => s,
+        _ => {
+            map.remove(&idx_rel_id.0);
+            return Ok(());
+        }
+    };
+    // the compound keys (key, field, sub_idx) of one tuple key are consecutive in the id -> key table
+    let mut ids: Vec<u32> = Vec::new();
+    for tk in tuple_keys {
+        let lo = staged.keys.partition_point(|x| x.0 < *tk);
+        ids.extend((lo..staged.keys.len()).take_while(|&i| staged.keys[i].0 == *tk).map(|i| i as u32));
+    }
+    if ids.is_empty() {
+        return Ok(());
+    }
+    let mut old_to_new = vec![0u32; staged.keys.len()];
+    let rc = unsafe { cozo_gpu_hnsw_remove(staged.h, ids.as_ptr(), ids.len() as u32) };
+    let rc = if rc == COZO_GPU_OK { unsafe { cozo_gpu_hnsw_compact(staged.h, old_to_new.as_mut_ptr()) } } else { rc };
+    if let Err(e) = check(rc) {
+        map.remove(&idx_rel_id.0); // the copy may be half updated: re-stage on the next search
+        return Err(e);
+    }
+    let mut id = 0usize;
+    staged.keys.retain(|_| {
+        id += 1;
+        old_to_new[id - 1] != COZO_GPU_NONE
+    });
     Ok(())
 }
 
