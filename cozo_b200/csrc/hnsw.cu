@@ -827,19 +827,10 @@ extern "C" int cozo_gpu_hnsw_stage(cozo_gpu_hnsw_t** out, const CozoGpuHnswStage
 extern "C" void cozo_gpu_hnsw_free(cozo_gpu_hnsw_t* h) {
   if (!h) return;
   for (auto* ws : h->pool) free_ws(ws);
-  if (h->d_vec && h->vec_owned) cudaFree(h->d_vec);
-  if (h->d_codes) cudaFree(h->d_codes);
+  const auto arrays = row_arrays(h);
+  for (size_t i = 0; i < arrays.size(); ++i)
+    if (arrays[i].ptr && (i != kVecArray || h->vec_owned)) cudaFree(arrays[i].ptr);
   if (h->d_vec64) cudaFree(h->d_vec64);
-  if (h->d_adj0) cudaFree(h->d_adj0);
-  if (h->d_upper_off) cudaFree(h->d_upper_off);
-  if (h->d_adj_up) cudaFree(h->d_adj_up);
-  if (h->d_adj0_dist) cudaFree(h->d_adj0_dist);
-  if (h->d_adj_up_dist) cudaFree(h->d_adj_up_dist);
-  if (h->d_node_level) cudaFree(h->d_node_level);
-  if (h->d_deg0) cudaFree(h->d_deg0);
-  if (h->d_deg_up) cudaFree(h->d_deg_up);
-  if (h->d_up_owner) cudaFree(h->d_up_owner);
-  if (h->d_dead) cudaFree(h->d_dead);
   delete h;
 }
 

@@ -111,15 +111,13 @@ struct SplitMix64 {
                        "%s failed: %s (line %d)", #call, cudaGetErrorString(_e), __LINE__);          \
   } while (0)
 
-// grow one device array to `new_elems` elements, keeping `old_elems`, filling the tail with `fill`
-template <class T>
-static int grow(T*& p, size_t old_elems, size_t new_elems, int fill_byte) {
-  T* np = nullptr;
-  H_CUDA(cudaMalloc(&np, std::max<size_t>(new_elems, 1) * sizeof(T)));
-  if (old_elems && p) H_CUDA(cudaMemcpy(np, p, old_elems * sizeof(T), cudaMemcpyDeviceToDevice));
-  if (new_elems > old_elems)
-    H_CUDA(cudaMemset(reinterpret_cast<char*>(np) + old_elems * sizeof(T), fill_byte, (new_elems - old_elems) * sizeof(T)));
-  if (p) cudaFree(p);
+// grow one device array to `new_bytes`, keeping `old_bytes`, filling the tail with `fill`; a borrowed array is not freed
+static int grow(void*& p, size_t old_bytes, size_t new_bytes, int fill_byte, bool owned = true) {
+  uint8_t* np = nullptr;
+  H_CUDA(cudaMalloc(&np, std::max<size_t>(new_bytes, 1)));
+  if (old_bytes && p) H_CUDA(cudaMemcpy(np, p, old_bytes, cudaMemcpyDeviceToDevice));
+  if (new_bytes > old_bytes) H_CUDA(cudaMemset(np + old_bytes, fill_byte, new_bytes - old_bytes));
+  if (p && owned) cudaFree(p);
   p = np;
   return 0;
 }
@@ -127,38 +125,34 @@ static int grow(T*& p, size_t old_elems, size_t new_elems, int fill_byte) {
 // capacity management: rows [0,n) / [0,up_rows) are live, the rest is pre-initialised slack
 int hnsw_reserve(cozo_gpu_hnsw* h, uint32_t need_n, uint64_t need_up) {
   HnswDev& g = h->dev;
+  const auto arrays = row_arrays(h);
   if (need_n > h->cap_n) {
     uint32_t nc = std::max<uint32_t>(need_n, (uint32_t)std::min<uint64_t>(0x7FFFFFFEull, (uint64_t)h->cap_n * 3 / 2));
-    if (!h->vec_owned) {
-      if (need_n > h->borrowed_rows) {  // borrowed vectors cannot grow in place: take a private copy
-        float* nv = nullptr;
-        H_CUDA(cudaMalloc(&nv, (size_t)nc * g.ld * 4));
-        if (g.n) H_CUDA(cudaMemcpy(nv, h->d_vec, (size_t)g.n * g.ld * 4, cudaMemcpyDeviceToDevice));
-        H_CUDA(cudaMemset(nv + (size_t)g.n * g.ld, 0, (size_t)(nc - g.n) * g.ld * 4));
-        h->d_vec = nv;
-        h->vec_owned = true;
+    for (size_t i = 0; i < arrays.size(); ++i) {
+      const RowArray& a = arrays[i];
+      int rc = 0;
+      if (a.upper) continue;
+      if (i == kCodesArray) {
+        hnsw_codes_reserve(h, nc);
+      } else if (i == kVecArray && !h->vec_owned) {
+        if (need_n > h->borrowed_rows) {  // borrowed vectors cannot grow in place: take a private copy
+          rc = grow(a.ptr, (size_t)g.n * a.row_bytes, (size_t)nc * a.row_bytes, a.fill, false);
+          if (!rc) h->vec_owned = true;
+        }
+      } else {
+        rc = grow(a.ptr, (size_t)h->cap_n * a.row_bytes, (size_t)nc * a.row_bytes, a.fill);
       }
-    } else {
-      int rc = grow(h->d_vec, (size_t)h->cap_n * g.ld, (size_t)nc * g.ld, 0);
       if (rc) return rc;
     }
-    hnsw_codes_reserve(h, nc);
-    int rc = grow(h->d_adj0, (size_t)h->cap_n * g.s0, (size_t)nc * g.s0, 0xFF);
-    if (!rc) rc = grow(h->d_adj0_dist, (size_t)h->cap_n * g.s0, (size_t)nc * g.s0, 0);
-    if (!rc) rc = grow(h->d_deg0, h->cap_n, nc, 0);
-    if (!rc) rc = grow(h->d_upper_off, h->cap_n, nc, 0xFF);
-    if (!rc) rc = grow(h->d_node_level, h->cap_n, nc, 0);
-    if (!rc) rc = grow(h->d_dead, h->cap_n, nc, 0);
-    if (rc) return rc;
     h->cap_n = nc;
   }
   if (need_up > h->cap_up || !h->d_adj_up) {
     uint64_t uc = std::max<uint64_t>(std::max<uint64_t>(need_up, 1), h->cap_up * 3 / 2);
-    int rc = grow(h->d_adj_up, (size_t)h->cap_up * g.su, (size_t)uc * g.su, 0xFF);
-    if (!rc) rc = grow(h->d_adj_up_dist, (size_t)h->cap_up * g.su, (size_t)uc * g.su, 0);
-    if (!rc) rc = grow(h->d_deg_up, (size_t)h->cap_up, (size_t)uc, 0);
-    if (!rc) rc = grow(h->d_up_owner, (size_t)h->cap_up, (size_t)uc, 0xFF);
-    if (rc) return rc;
+    for (const RowArray& a : arrays) {
+      if (!a.upper) continue;
+      int rc = grow(a.ptr, (size_t)h->cap_up * a.row_bytes, (size_t)uc * a.row_bytes, a.fill);
+      if (rc) return rc;
+    }
     h->cap_up = uc;
   }
   g.vec = h->d_vec;
@@ -166,6 +160,11 @@ int hnsw_reserve(cozo_gpu_hnsw* h, uint32_t need_n, uint64_t need_up) {
   g.adj_up = h->d_adj_up;
   g.upper_off = h->d_upper_off;
   return 0;
+}
+
+// never write into a borrowed vector buffer: take a private copy first
+static int own_vectors(cozo_gpu_hnsw* h) {
+  return h->vec_owned ? 0 : hnsw_reserve(h, h->borrowed_rows + 1, h->up_rows);
 }
 
 static BuildDev build_dev(cozo_gpu_hnsw* h) {
@@ -198,31 +197,20 @@ int hnsw_ensure_build_state(cozo_gpu_hnsw* h) {
     // everything below the capacity as initialised (a capacity of 1 with 0 live upper rows would carry one
     // row of uninitialised ids and degrees into the grown arrays)
     h->cap_up = h->up_rows;
-    uint32_t* p32 = nullptr;
-    float* pf = nullptr;
-    uint8_t* p8 = nullptr;
-    const size_t up_alloc = std::max<size_t>((size_t)h->cap_up, 1);
-    H_CUDA(cudaMalloc(&pf, std::max<size_t>((size_t)h->cap_n * g.s0, 1) * 4));
-    h->d_adj0_dist = pf;
-    H_CUDA(cudaMalloc(&pf, up_alloc * g.su * 4));
-    h->d_adj_up_dist = pf;
-    H_CUDA(cudaMalloc(&p32, std::max<size_t>(h->cap_n, 1) * 4));
-    h->d_deg0 = p32;
-    H_CUDA(cudaMalloc(&p32, up_alloc * 4));
-    h->d_deg_up = p32;
-    H_CUDA(cudaMalloc(&p32, up_alloc * 4));
-    h->d_up_owner = p32;
-    H_CUDA(cudaMalloc(&p8, std::max<size_t>(h->cap_n, 1)));
-    h->d_node_level = p8;
-    H_CUDA(cudaMalloc(&p8, std::max<size_t>(h->cap_n, 1)));
-    h->d_dead = p8;
-    H_CUDA(cudaMemset(h->d_dead, 0, std::max<size_t>(h->cap_n, 1)));
+    // staging made vec, codes, adj0, upper_off and adj_up; the builder's arrays start as unused capacity
+    const auto arrays = row_arrays(h);
+    for (size_t i = 0; i < arrays.size(); ++i) {
+      const RowArray& a = arrays[i];
+      if (a.ptr || i == kVecArray || i == kCodesArray) continue;
+      const size_t bytes = std::max<size_t>(a.upper ? h->cap_up : h->cap_n, 1) * a.row_bytes;
+      H_CUDA(cudaMalloc(&a.ptr, bytes));
+      H_CUDA(cudaMemset(a.ptr, a.fill, bytes));
+    }
     if (g.n) H_CUDA(cudaMemcpy(h->d_node_level, h->node_level.data(), g.n, cudaMemcpyHostToDevice));
-    std::vector<uint32_t> owner(up_alloc, NONE);
-    uint64_t r = 0;
+    std::vector<uint32_t> owner;
     for (uint32_t i = 0; i < g.n; ++i)
-      for (uint32_t L = 0; L < h->node_level[i]; ++L) owner[r++] = i;
-    H_CUDA(cudaMemcpy(h->d_up_owner, owner.data(), up_alloc * 4, cudaMemcpyHostToDevice));
+      for (uint32_t L = 0; L < h->node_level[i]; ++L) owner.push_back(i);
+    if (!owner.empty()) H_CUDA(cudaMemcpy(h->d_up_owner, owner.data(), owner.size() * 4, cudaMemcpyHostToDevice));
     h->live.assign(g.n, 1);
     h->n_live = g.n;
   }
@@ -485,9 +473,9 @@ int hnsw_insert_range(cozo_gpu_hnsw* h, uint32_t begin, uint32_t end, uint32_t m
 
 // levels of `count` new rows, drawn in row order from the handle's seeded level law (hnsw.rs:46-52),
 // level_multiplier = 1/ln(m) (relation.rs:1147)
-static std::vector<uint8_t> draw_levels(cozo_gpu_hnsw* h, uint32_t count) {
-  SplitMix64 rng{h->rng_state};
-  const double mult = 1.0 / std::log((double)h->m_max);
+static std::vector<uint8_t> draw_levels(uint64_t& rng_state, uint32_t m_max, uint32_t count) {
+  SplitMix64 rng{rng_state};
+  const double mult = 1.0 / std::log((double)m_max);
   std::vector<uint8_t> lv(count);
   for (uint32_t i = 0; i < count; ++i) {
     double u = rng.uniform();
@@ -495,7 +483,7 @@ static std::vector<uint8_t> draw_levels(cozo_gpu_hnsw* h, uint32_t count) {
     if (!(r < 15.0)) r = 15.0;
     lv[i] = (uint8_t)std::floor(r);
   }
-  h->rng_state = rng.s;
+  rng_state = rng.s;
   return lv;
 }
 
@@ -504,7 +492,7 @@ static int append_nodes(cozo_gpu_hnsw* h, const float* vectors, int on_device, u
   HnswDev& g = h->dev;
   const uint32_t n0 = g.n, n1 = n0 + count;
   if ((uint64_t)n0 + count >= 0x7FFFFFFFull) return set_error(COZO_GPU_EUNSUP, "too many vectors");
-  const std::vector<uint8_t> lvs = draw_levels(h, count);
+  const std::vector<uint8_t> lvs = draw_levels(h->rng_state, h->m_max, count);
   h->node_level.resize(n1, 0);
   h->live.resize(n1, 1);
   std::vector<uint32_t> upper_off(count, NONE);
@@ -626,41 +614,117 @@ extern "C" int cozo_gpu_hnsw_insert(cozo_gpu_hnsw_t* h, const float* vectors, ui
   return hnsw_insert_range(h, n0, n0 + count, 0);
 }
 
-// Moves rows [first, n) of one per-node array (row_bytes each) to their relabelled rows, `chunk` rows at a time from the
-// tail through `stage`.  Destinations are never below their sources, so a chunk only overwrites rows already moved, and
-// no second copy of the array is needed.  On the legacy default stream.
-static int shift_rows(void* base, size_t row_bytes, uint32_t first, uint32_t n, uint8_t* stage, uint64_t chunk,
-                      const uint32_t* d_pos, uint32_t npos) {
-  uint8_t* p = static_cast<uint8_t*>(base);
-  for (uint32_t hi = n; hi > first;) {
-    const uint32_t lo = hi - (uint32_t)std::min<uint64_t>(chunk, hi - first);
-    const uint32_t rows = hi - lo;
-    H_CUDA(cudaMemcpyAsync(stage, p + (size_t)lo * row_bytes, (size_t)rows * row_bytes, cudaMemcpyDeviceToDevice, 0));
-    if (row_bytes % 16 == 0) {
-      const uint32_t e = (uint32_t)(row_bytes / 16);
-      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
-      shift_rows_kernel<uint4><<<(uint32_t)((threads + 255) / 256), 256>>>(
-          reinterpret_cast<const uint4*>(stage), reinterpret_cast<uint4*>(p), e, lo, rows, d_pos, npos);
-    } else if (row_bytes % 4 == 0) {
-      const uint32_t e = (uint32_t)(row_bytes / 4);
-      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
-      shift_rows_kernel<uint32_t><<<(uint32_t)((threads + 255) / 256), 256>>>(
-          reinterpret_cast<const uint32_t*>(stage), reinterpret_cast<uint32_t*>(p), e, lo, rows, d_pos, npos);
-    } else {
-      const uint32_t e = (uint32_t)row_bytes;
-      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
-      shift_rows_kernel<uint8_t><<<(uint32_t)((threads + 255) / 256), 256>>>(stage, p, e, lo, rows, d_pos, npos);
-    }
+// a device allocation freed at the end of the scope
+template <class T>
+struct DevScratch {
+  T* p = nullptr;
+  ~DevScratch() {
+    if (p) cudaFree(p);
+  }
+};
+
+template <class T, class Map>
+static void launch_move_rows(const uint8_t* stage, uint8_t* base, size_t row_bytes, uint32_t lo, uint32_t rows, Map map) {
+  const uint32_t e = (uint32_t)(row_bytes / sizeof(T));
+  const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
+  move_rows_kernel<T, Map><<<(uint32_t)((threads + 255) / 256), 256>>>(reinterpret_cast<const T*>(stage),
+                                                                         reinterpret_cast<T*>(base), e, lo, rows, map);
+}
+
+// Moves rows [first, n) of one array to rows map(j), dropping rows that map to NONE, `chunk` rows at a time through
+// `stage`: from the tail when destinations are above their sources, from the head when they are below.  Either way a
+// chunk only overwrites rows already read, so no second copy of the array is needed.  On the legacy default stream.
+template <class Map>
+static int move_rows(const RowArray& a, uint32_t first, uint32_t n, bool tail_first, uint8_t* stage, uint64_t chunk,
+                     Map map) {
+  uint8_t* p = static_cast<uint8_t*>(a.ptr);
+  const size_t rb = a.row_bytes;
+  for (uint32_t done = 0; done < n - first;) {
+    const uint32_t rows = (uint32_t)std::min<uint64_t>(chunk, n - first - done);
+    const uint32_t lo = tail_first ? n - done - rows : first + done;
+    H_CUDA(cudaMemcpyAsync(stage, p + (size_t)lo * rb, (size_t)rows * rb, cudaMemcpyDeviceToDevice, 0));
+    if (rb % 16 == 0) launch_move_rows<uint4>(stage, p, rb, lo, rows, map);
+    else if (rb % 4 == 0) launch_move_rows<uint32_t>(stage, p, rb, lo, rows, map);
+    else launch_move_rows<uint8_t>(stage, p, rb, lo, rows, map);
     H_CUDA(cudaGetLastError());
-    hi = lo;
+    done += rows;
   }
   return 0;
 }
 
-static int relabel_ids(uint32_t* ids, size_t count, const uint32_t* d_pos, uint32_t npos) {
+template <class Map>
+static int map_ids(uint32_t* ids, size_t count, Map map, uint32_t* bad) {
   if (!count) return 0;
-  relabel_ids_kernel<<<(uint32_t)((count + 255) / 256), 256>>>(ids, count, d_pos, npos);
+  map_ids_kernel<Map><<<(uint32_t)((count + 255) / 256), 256>>>(ids, count, map, bad);
   H_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Applies a monotone relabelling to the handle.  Node row j >= first moves to row node_map(j) (host_map[j] on the host;
+// NONE drops the row) and n1 node rows remain.  With up_map, upper row r >= up_first likewise moves to up_map[r] and up1
+// upper rows remain; without it the upper rows stay where they are.  Every row array moves through one staging buffer
+// in chunks of 64 MB, or of `hnsw.shift_chunk_rows` rows when that is set; then every stored id is mapped, rows freed
+// at the end return to the state of unused capacity, and the host copies of levels, live flags and the entry follow.
+// The caller has made room for n1 rows.  All scratch is allocated before any row moves, so that running out of memory
+// leaves the index as it was.
+template <class NodeMap>
+static int relabel_rows(cozo_gpu_hnsw* h, NodeMap node_map, const std::vector<uint32_t>& host_map, uint32_t first,
+                        uint32_t n1, const uint32_t* up_map = nullptr, uint32_t up_first = 0, uint32_t up1 = 0) {
+  HnswDev& g = h->dev;
+  const uint32_t n0 = g.n, up0 = (uint32_t)h->up_rows;
+  if (!up_map) up_first = up1 = up0;
+  const size_t kStageBytes = (size_t)64 << 20;
+  const int64_t chunk_opt = get_option("hnsw.shift_chunk_rows", 0);
+  auto chunk_rows = [&](const RowArray& a) {
+    const uint64_t moving = a.upper ? up0 - up_first : n0 - first;
+    const uint64_t c = chunk_opt > 0 ? (uint64_t)chunk_opt : std::max<uint64_t>(1, kStageBytes / a.row_bytes);
+    return std::max<uint64_t>(1, std::min(c, moving));
+  };
+  size_t stage_bytes = 1;
+  for (const RowArray& a : row_arrays(h)) stage_bytes = std::max(stage_bytes, (size_t)chunk_rows(a) * a.row_bytes);
+  DevScratch<uint8_t> stage;
+  DevScratch<uint32_t> bad;  // stored ids that name a dropped row
+  H_CUDA(cudaMalloc(&stage.p, stage_bytes));
+  H_CUDA(cudaMalloc(&bad.p, 4));
+  H_CUDA(cudaMemsetAsync(bad.p, 0, 4, 0));
+  int rc = own_vectors(h);
+  if (rc) return rc;
+
+  // after the private copy: the arrays' current addresses
+  const auto arrays = row_arrays(h);
+  for (const RowArray& a : arrays) {
+    if (!a.ptr) continue;
+    const uint64_t chunk = chunk_rows(a);
+    rc = a.upper ? move_rows(a, up_first, up0, up1 > up0, stage.p, chunk, TableMap{up_map})
+                 : move_rows(a, first, n0, n1 > n0, stage.p, chunk, node_map);
+    if (rc) return rc;
+  }
+  rc = map_ids(h->d_adj0, (size_t)n1 * g.s0, node_map, bad.p);
+  if (!rc) rc = map_ids(h->d_adj_up, (size_t)up1 * g.su, node_map, bad.p);
+  if (!rc) rc = map_ids(h->d_up_owner, up1, node_map, bad.p);
+  if (!rc && up_map) rc = map_ids(h->d_upper_off, n1, TableMap{up_map}, bad.p);
+  if (rc) return rc;
+  for (const RowArray& a : arrays) {
+    const uint32_t from = a.upper ? up1 : n1, to = a.upper ? up0 : n0;
+    if (a.ptr && from < to)
+      H_CUDA(cudaMemsetAsync(static_cast<uint8_t*>(a.ptr) + (size_t)from * a.row_bytes, a.fill,
+                             (size_t)(to - from) * a.row_bytes, 0));
+  }
+  // the host copies, built while the device works
+  std::vector<uint8_t> level(n1), live(n1, 1);
+  for (uint32_t j = 0; j < n0; ++j)
+    if (host_map[j] != NONE) {
+      level[host_map[j]] = h->node_level[j];
+      live[host_map[j]] = h->live[j];
+    }
+  uint32_t nbad = 0;
+  H_CUDA(cudaMemcpy(&nbad, bad.p, 4, cudaMemcpyDeviceToHost));
+  if (nbad) return set_error(COZO_GPU_ECUDA, "internal: %u stored ids name removed ids", nbad);
+  h->node_level.swap(level);
+  h->live.swap(live);
+  if (g.entry != NONE) g.entry = host_map[g.entry];
+  h->up_rows = up1;
+  g.n = n1;
   return 0;
 }
 
@@ -694,42 +758,18 @@ extern "C" int cozo_gpu_hnsw_insert_at(cozo_gpu_hnsw_t* h, const uint32_t* posit
   if (rc) return rc;
 
   // scratch first, so that running out of memory leaves the index as it was
-  struct Scratch {
-    uint32_t *pos = nullptr, *ids = nullptr, *up_off = nullptr;
-    uint8_t *levels = nullptr, *stage = nullptr;
-    float* vec = nullptr;
-    ~Scratch() {
-      void* ptrs[] = {pos, ids, up_off, levels, stage, vec};
-      for (void* p : ptrs)
-        if (p) cudaFree(p);
-    }
-  } sc;
-  H_CUDA(cudaMalloc(&sc.pos, (size_t)count * 4));
-  H_CUDA(cudaMalloc(&sc.ids, (size_t)count * 4));
-  H_CUDA(cudaMalloc(&sc.up_off, (size_t)count * 4));
-  H_CUDA(cudaMalloc(&sc.levels, count));
-  if (!vectors_on_device) H_CUDA(cudaMalloc(&sc.vec, (size_t)count * g.dim * 4));
-  // Per-node arrays and their row sizes (code rows only where the index has them).  Each array moves through the
-  // staging buffer in chunks of kStageBytes / row_bytes rows, or of `hnsw.shift_chunk_rows` rows when that is set.
-  const size_t kStageBytes = (size_t)64 << 20;
-  const size_t vec_row = (size_t)g.ld * 4, adj_row = (size_t)g.s0 * 4;
-  const size_t row_bytes[] = {vec_row, g.code_ld, adj_row, adj_row, 4, 4, 1, 1};
-  const int64_t chunk_opt = get_option("hnsw.shift_chunk_rows", 0);
-  const uint64_t moving = n0 - positions[0];
-  auto chunk_rows = [&](size_t rb) {
-    const uint64_t c = chunk_opt > 0 ? (uint64_t)chunk_opt : std::max<uint64_t>(1, kStageBytes / rb);
-    return std::max<uint64_t>(1, std::min(c, moving));
-  };
-  size_t stage_bytes = 1;
-  for (size_t rb : row_bytes) stage_bytes = std::max(stage_bytes, (size_t)chunk_rows(rb) * rb);
-  H_CUDA(cudaMalloc(&sc.stage, stage_bytes));
+  DevScratch<uint32_t> d_pos, d_ids, d_up_off;
+  DevScratch<uint8_t> d_levels;
+  DevScratch<float> d_vec;
+  H_CUDA(cudaMalloc(&d_pos.p, (size_t)count * 4));
+  H_CUDA(cudaMalloc(&d_ids.p, (size_t)count * 4));
+  H_CUDA(cudaMalloc(&d_up_off.p, (size_t)count * 4));
+  H_CUDA(cudaMalloc(&d_levels.p, count));
+  if (!vectors_on_device) H_CUDA(cudaMalloc(&d_vec.p, (size_t)count * g.dim * 4));
 
-  if (!h->vec_owned) {  // never write into a borrowed buffer
-    rc = hnsw_reserve(h, h->borrowed_rows + 1, h->up_rows);
-    if (rc) return rc;
-  }
   const uint32_t n1 = n0 + count;
-  const std::vector<uint8_t> lvs = draw_levels(h, count);
+  uint64_t rng = h->rng_state;  // kept until the rows have moved
+  const std::vector<uint8_t> lvs = draw_levels(rng, h->m_max, count);
   std::vector<uint32_t> new_ids(count), up_off(count, NONE), owners;
   uint64_t up = h->up_rows;
   for (uint32_t i = 0; i < count; ++i) {
@@ -740,96 +780,42 @@ extern "C" int cozo_gpu_hnsw_insert_at(cozo_gpu_hnsw_t* h, const uint32_t* posit
       for (uint32_t L = 0; L < lvs[i]; ++L) owners.push_back(new_ids[i]);
     }
   }
+  // old row j -> j + #{positions <= j}; rows below positions[0] stay
+  std::vector<uint32_t> map(n0);
+  for (uint32_t j = 0, i = 0; j < n0; ++j) {
+    while (i < count && positions[i] <= j) ++i;
+    map[j] = j + i;
+  }
   const uint64_t up0 = h->up_rows;
   rc = hnsw_reserve(h, n1, up);
   if (rc) return rc;
-  H_CUDA(cudaMemcpy(sc.pos, positions, (size_t)count * 4, cudaMemcpyHostToDevice));
-  H_CUDA(cudaMemcpy(sc.ids, new_ids.data(), (size_t)count * 4, cudaMemcpyHostToDevice));
-  H_CUDA(cudaMemcpy(sc.up_off, up_off.data(), (size_t)count * 4, cudaMemcpyHostToDevice));
-  H_CUDA(cudaMemcpy(sc.levels, lvs.data(), count, cudaMemcpyHostToDevice));
+  H_CUDA(cudaMemcpy(d_pos.p, positions, (size_t)count * 4, cudaMemcpyHostToDevice));
+  H_CUDA(cudaMemcpy(d_ids.p, new_ids.data(), (size_t)count * 4, cudaMemcpyHostToDevice));
+  H_CUDA(cudaMemcpy(d_up_off.p, up_off.data(), (size_t)count * 4, cudaMemcpyHostToDevice));
+  H_CUDA(cudaMemcpy(d_levels.p, lvs.data(), count, cudaMemcpyHostToDevice));
   const float* d_new_vec = vectors;
   if (!vectors_on_device) {
-    H_CUDA(cudaMemcpy(sc.vec, vectors, (size_t)count * g.dim * 4, cudaMemcpyHostToDevice));
-    d_new_vec = sc.vec;
+    H_CUDA(cudaMemcpy(d_vec.p, vectors, (size_t)count * g.dim * 4, cudaMemcpyHostToDevice));
+    d_new_vec = d_vec.p;
   }
-
-  // 1. every per-node array: old row j -> j + #{positions <= j}; rows below positions[0] stay
-  void* const bases[] = {h->d_vec, g.codes ? h->d_codes : nullptr, h->d_adj0, h->d_adj0_dist,
-                         h->d_deg0, h->d_upper_off, h->d_node_level, h->d_dead};
-  for (size_t a = 0; a < 8; ++a) {
-    if (!bases[a]) continue;
-    rc = shift_rows(bases[a], row_bytes[a], positions[0], n0, sc.stage, chunk_rows(row_bytes[a]), sc.pos, count);
-    if (rc) return rc;
-  }
-  // 2. the new rows
-  place_new_rows_kernel<<<(uint32_t)(((uint64_t)count * 32 + 255) / 256), 256>>>(
-      sc.ids, count, d_new_vec, g.dim, h->d_vec, g.ld, h->d_adj0, g.s0, h->d_deg0, sc.up_off, h->d_upper_off,
-      sc.levels, h->d_node_level, h->d_dead);
-  H_CUDA(cudaGetLastError());
-  hnsw_codes_fill(h, 0, count, sc.ids);
-  // 3. every stored id; adj_up rows stay where they are (upper_off holds row numbers)
-  rc = relabel_ids(h->d_adj0, (size_t)n1 * g.s0, sc.pos, count);
-  if (!rc) rc = relabel_ids(h->d_adj_up, (size_t)up0 * g.su, sc.pos, count);
-  if (!rc) rc = relabel_ids(h->d_up_owner, (size_t)up0, sc.pos, count);
+  // adj_up rows stay where they are (upper_off holds row numbers)
+  rc = relabel_rows(h, GapMap{d_pos.p, count}, map, positions[0], n1);
   if (rc) return rc;
+  h->rng_state = rng;
+  // the new rows; their upper rows are fresh rows at the end of adj_up
+  place_new_rows_kernel<<<(uint32_t)(((uint64_t)count * 32 + 255) / 256), 256>>>(
+      d_ids.p, count, d_new_vec, g.dim, h->d_vec, g.ld, h->d_adj0, g.s0, h->d_deg0, d_up_off.p, h->d_upper_off,
+      d_levels.p, h->d_node_level, h->d_dead);
+  H_CUDA(cudaGetLastError());
+  hnsw_codes_fill(h, 0, count, d_ids.p);
   if (!owners.empty())
     H_CUDA(cudaMemcpyAsync(h->d_up_owner + up0, owners.data(), owners.size() * 4, cudaMemcpyHostToDevice, 0));
   H_CUDA(cudaDeviceSynchronize());  // the builder runs on a workspace stream, which the legacy stream does not order
-
-  // host copies
-  std::vector<uint8_t> level(n1), live(n1, 1);
-  for (uint32_t j = 0, i = 0; j < n0; ++j) {
-    while (i < count && positions[i] <= j) ++i;
-    level[j + i] = h->node_level[j];
-    live[j + i] = h->live[j];
-  }
-  for (uint32_t i = 0; i < count; ++i) level[new_ids[i]] = lvs[i];
-  h->node_level.swap(level);
-  h->live.swap(live);
-  if (g.entry != NONE)
-    g.entry += (uint32_t)(std::upper_bound(positions, positions + count, g.entry) - positions);
+  for (uint32_t i = 0; i < count; ++i) h->node_level[new_ids[i]] = lvs[i];
   h->up_rows = up;
-  g.n = n1;
   rc = hnsw_insert_ids(h, new_ids, 0, true);
   if (rc) return rc;
   if (out_ids) std::copy(new_ids.begin(), new_ids.end(), out_ids);
-  return 0;
-}
-
-// Moves rows [first, n) of one array (row_bytes each) to rows map[j], dropping rows that map to NONE, `chunk` rows at a
-// time from the head through `stage`.  Destinations are never above their sources, so a chunk only overwrites rows
-// already read, and no second copy of the array is needed.  On the legacy default stream.
-static int compact_rows(void* base, size_t row_bytes, uint32_t first, uint32_t n, uint8_t* stage, uint64_t chunk,
-                        const uint32_t* d_map) {
-  uint8_t* p = static_cast<uint8_t*>(base);
-  for (uint32_t lo = first; lo < n;) {
-    const uint32_t rows = (uint32_t)std::min<uint64_t>(chunk, n - lo);
-    H_CUDA(cudaMemcpyAsync(stage, p + (size_t)lo * row_bytes, (size_t)rows * row_bytes, cudaMemcpyDeviceToDevice, 0));
-    if (row_bytes % 16 == 0) {
-      const uint32_t e = (uint32_t)(row_bytes / 16);
-      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
-      compact_rows_kernel<uint4><<<(uint32_t)((threads + 255) / 256), 256>>>(
-          reinterpret_cast<const uint4*>(stage), reinterpret_cast<uint4*>(p), e, lo, rows, d_map);
-    } else if (row_bytes % 4 == 0) {
-      const uint32_t e = (uint32_t)(row_bytes / 4);
-      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
-      compact_rows_kernel<uint32_t><<<(uint32_t)((threads + 255) / 256), 256>>>(
-          reinterpret_cast<const uint32_t*>(stage), reinterpret_cast<uint32_t*>(p), e, lo, rows, d_map);
-    } else {
-      const uint32_t e = (uint32_t)row_bytes;
-      const uint64_t threads = (uint64_t)rows * (e >= 32 ? 32 : 1);
-      compact_rows_kernel<uint8_t><<<(uint32_t)((threads + 255) / 256), 256>>>(stage, p, e, lo, rows, d_map);
-    }
-    H_CUDA(cudaGetLastError());
-    lo += rows;
-  }
-  return 0;
-}
-
-static int compact_ids(uint32_t* ids, size_t count, const uint32_t* d_map, uint32_t* d_bad) {
-  if (!count) return 0;
-  compact_ids_kernel<<<(uint32_t)((count + 255) / 256), 256>>>(ids, count, d_map, d_bad);
-  H_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -859,104 +845,31 @@ extern "C" int cozo_gpu_hnsw_compact(cozo_gpu_hnsw_t* h, uint32_t* old_to_new) {
   const uint32_t up0 = (uint32_t)h->up_rows;
 
   // scratch first, so that running out of memory leaves the index as it was
-  struct Scratch {
-    uint32_t *map = nullptr, *keep = nullptr, *up_map = nullptr, *counters = nullptr;
-    uint8_t* stage = nullptr;
-    void* cub_tmp = nullptr;
-    ~Scratch() {
-      void* ptrs[] = {map, keep, up_map, counters, stage, cub_tmp};
-      for (void* p : ptrs)
-        if (p) cudaFree(p);
-    }
-  } sc;
-  H_CUDA(cudaMalloc(&sc.map, (size_t)n0 * 4));
-  H_CUDA(cudaMalloc(&sc.keep, ((size_t)up0 + 1) * 4));
-  H_CUDA(cudaMalloc(&sc.up_map, ((size_t)up0 + 1) * 4));
-  H_CUDA(cudaMalloc(&sc.counters, 8));
+  DevScratch<uint32_t> d_map, keep, up_map, first_drop;
+  DevScratch<uint8_t> cub_tmp;
+  H_CUDA(cudaMalloc(&d_map.p, (size_t)n0 * 4));
+  H_CUDA(cudaMalloc(&keep.p, ((size_t)up0 + 1) * 4));
+  H_CUDA(cudaMalloc(&up_map.p, ((size_t)up0 + 1) * 4));
+  H_CUDA(cudaMalloc(&first_drop.p, 4));
   size_t cub_bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, sc.keep, sc.up_map, (int)(up0 + 1));
-  H_CUDA(cudaMalloc(&sc.cub_tmp, std::max<size_t>(cub_bytes, 16)));
-  H_CUDA(cudaMemcpy(sc.map, map.data(), (size_t)n0 * 4, cudaMemcpyHostToDevice));
-  // counters[0]: first dropped upper row (NONE: none), counters[1]: stored ids that name a removed id
-  H_CUDA(cudaMemset(sc.counters, 0xFF, 4));
-  H_CUDA(cudaMemset(sc.counters + 1, 0, 4));
+  cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, keep.p, up_map.p, (int)(up0 + 1));
+  H_CUDA(cudaMalloc(&cub_tmp.p, std::max<size_t>(cub_bytes, 16)));
+  H_CUDA(cudaMemcpy(d_map.p, map.data(), (size_t)n0 * 4, cudaMemcpyHostToDevice));
+  H_CUDA(cudaMemset(first_drop.p, 0xFF, 4));  // NONE: no upper row is dropped
   // the upper-row map: rows whose owner stays, in row order
-  upper_keep_kernel<<<(up0 + 256) / 256, 256>>>(h->d_up_owner, up0, sc.map, sc.keep);
+  upper_keep_kernel<<<(up0 + 256) / 256, 256>>>(h->d_up_owner, up0, d_map.p, keep.p);
   H_CUDA(cudaGetLastError());
-  cub::DeviceScan::ExclusiveSum(sc.cub_tmp, cub_bytes, sc.keep, sc.up_map, (int)(up0 + 1));
-  if (up0) upper_map_kernel<<<(up0 + 255) / 256, 256>>>(sc.keep, up0, sc.up_map, sc.counters);
+  cub::DeviceScan::ExclusiveSum(cub_tmp.p, cub_bytes, keep.p, up_map.p, (int)(up0 + 1));
+  if (up0) upper_map_kernel<<<(up0 + 255) / 256, 256>>>(keep.p, up0, up_map.p, first_drop.p);
   H_CUDA(cudaGetLastError());
   uint32_t up1 = 0, up_first = NONE;
-  H_CUDA(cudaMemcpy(&up1, sc.up_map + up0, 4, cudaMemcpyDeviceToHost));
-  H_CUDA(cudaMemcpy(&up_first, sc.counters, 4, cudaMemcpyDeviceToHost));
+  H_CUDA(cudaMemcpy(&up1, up_map.p + up0, 4, cudaMemcpyDeviceToHost));
+  H_CUDA(cudaMemcpy(&up_first, first_drop.p, 4, cudaMemcpyDeviceToHost));
   if (up_first == NONE) up_first = up0;
 
-  // Per-node and upper-row arrays with their row sizes (code rows only where the index has them).  Each array moves
-  // through the staging buffer in chunks of kStageBytes / row_bytes rows, or of `hnsw.shift_chunk_rows` rows when that
-  // is set.
-  const size_t kStageBytes = (size_t)64 << 20;
-  const size_t vec_row = (size_t)g.ld * 4, adj_row = (size_t)g.s0 * 4, up_row = (size_t)g.su * 4;
-  const size_t row_bytes[] = {vec_row, g.code_ld, adj_row, adj_row, 4, 4, 1, 1, up_row, up_row, 4, 4};
-  constexpr size_t kNodeArrays = 8, kArrays = 12;
-  const int64_t chunk_opt = get_option("hnsw.shift_chunk_rows", 0);
-  auto chunk_rows = [&](size_t a) {
-    const uint64_t moving = a < kNodeArrays ? n0 - first : up0 - up_first;
-    const uint64_t c = chunk_opt > 0 ? (uint64_t)chunk_opt : std::max<uint64_t>(1, kStageBytes / row_bytes[a]);
-    return std::max<uint64_t>(1, std::min(c, moving));
-  };
-  size_t stage_bytes = 1;
-  for (size_t a = 0; a < kArrays; ++a) stage_bytes = std::max(stage_bytes, (size_t)chunk_rows(a) * row_bytes[a]);
-  H_CUDA(cudaMalloc(&sc.stage, stage_bytes));
-
-  if (!h->vec_owned) {  // never write into a borrowed buffer
-    rc = hnsw_reserve(h, h->borrowed_rows + 1, h->up_rows);
-    if (rc) return rc;
-  }
-  // after the private copy: the arrays' current addresses
-  void* const moved[] = {h->d_vec, g.codes ? h->d_codes : nullptr, h->d_adj0, h->d_adj0_dist, h->d_deg0,
-                         h->d_upper_off, h->d_node_level, h->d_dead, h->d_adj_up, h->d_adj_up_dist, h->d_deg_up,
-                         h->d_up_owner};
-  // 1. every array: kept rows move down, rows before the first dropped one stay
-  for (size_t a = 0; a < kArrays; ++a) {
-    if (!moved[a]) continue;
-    rc = a < kNodeArrays ? compact_rows(moved[a], row_bytes[a], first, n0, sc.stage, chunk_rows(a), sc.map)
-                         : compact_rows(moved[a], row_bytes[a], up_first, up0, sc.stage, chunk_rows(a), sc.up_map);
-    if (rc) return rc;
-  }
-  // 2. every stored id of a kept row: node ids through the node map, upper_off through the row map
-  rc = compact_ids(h->d_adj0, (size_t)n1 * g.s0, sc.map, sc.counters + 1);
-  if (!rc) rc = compact_ids(h->d_adj_up, (size_t)up1 * g.su, sc.map, sc.counters + 1);
-  if (!rc) rc = compact_ids(h->d_up_owner, up1, sc.map, sc.counters + 1);
-  if (!rc) rc = compact_ids(h->d_upper_off, n1, sc.up_map, sc.counters + 1);
+  rc = relabel_rows(h, TableMap{d_map.p}, map, first, n1, up_map.p, up_first, up1);
   if (rc) return rc;
-  // 3. the freed rows go back to the state of unused capacity, which append_nodes expects
-  H_CUDA(cudaMemsetAsync(h->d_vec + (size_t)n1 * g.ld, 0, (size_t)(n0 - n1) * vec_row, 0));
-  H_CUDA(cudaMemsetAsync(h->d_adj0 + (size_t)n1 * g.s0, 0xFF, (size_t)(n0 - n1) * adj_row, 0));
-  H_CUDA(cudaMemsetAsync(h->d_adj0_dist + (size_t)n1 * g.s0, 0, (size_t)(n0 - n1) * adj_row, 0));
-  H_CUDA(cudaMemsetAsync(h->d_deg0 + n1, 0, (size_t)(n0 - n1) * 4, 0));
-  H_CUDA(cudaMemsetAsync(h->d_upper_off + n1, 0xFF, (size_t)(n0 - n1) * 4, 0));
-  H_CUDA(cudaMemsetAsync(h->d_node_level + n1, 0, n0 - n1, 0));
-  H_CUDA(cudaMemsetAsync(h->d_dead + n1, 0, n0 - n1, 0));
-  if (up1 < up0) {
-    H_CUDA(cudaMemsetAsync(h->d_adj_up + (size_t)up1 * g.su, 0xFF, (size_t)(up0 - up1) * up_row, 0));
-    H_CUDA(cudaMemsetAsync(h->d_adj_up_dist + (size_t)up1 * g.su, 0, (size_t)(up0 - up1) * up_row, 0));
-    H_CUDA(cudaMemsetAsync(h->d_deg_up + up1, 0, (size_t)(up0 - up1) * 4, 0));
-    H_CUDA(cudaMemsetAsync(h->d_up_owner + up1, 0xFF, (size_t)(up0 - up1) * 4, 0));
-  }
-  uint32_t bad = 0;
-  H_CUDA(cudaMemcpy(&bad, sc.counters + 1, 4, cudaMemcpyDeviceToHost));
-  if (bad) return set_error(COZO_GPU_ECUDA, "internal: %u stored ids name removed ids", bad);
-
-  // host copies
-  std::vector<uint8_t> level(n1);
-  for (uint32_t j = 0; j < n0; ++j)
-    if (map[j] != NONE) level[map[j]] = h->node_level[j];
-  h->node_level.swap(level);
-  h->live.assign(n1, 1);
   h->n_live = n1;
-  if (g.entry != NONE) g.entry = map[g.entry];
-  h->up_rows = up1;
-  g.n = n1;
   if (old_to_new) std::copy(map.begin(), map.end(), old_to_new);
   return 0;
 }
@@ -1042,10 +955,8 @@ extern "C" int cozo_gpu_hnsw_update(cozo_gpu_hnsw_t* h, const uint32_t* ids, con
     if (rc) return rc;
   }
   // 2. new payloads, revive
-  if (!h->vec_owned) {  // never write into a borrowed buffer
-    rc = hnsw_reserve(h, h->borrowed_rows + 1, h->up_rows);
-    if (rc) return rc;
-  }
+  rc = own_vectors(h);
+  if (rc) return rc;
   for (uint32_t i = 0; i < count; ++i)
     H_CUDA(cudaMemcpy(h->d_vec + (size_t)ids[i] * g.ld, vectors + (size_t)i * g.dim, (size_t)g.dim * 4,
                       cudaMemcpyHostToDevice));

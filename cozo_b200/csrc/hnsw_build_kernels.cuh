@@ -579,38 +579,56 @@ __global__ void mark_dead_kernel(const uint32_t* ids, uint32_t count, uint8_t* d
   if (i < count) dead[ids[i]] = 1;
 }
 
-// ---- insert at any key position (cozo_gpu_hnsw_insert_at) -------------------------------------------------------
-// pos: the ascending insert positions.  Old id j becomes j + #{i : pos[i] <= j}.
-__device__ __forceinline__ uint32_t relabel_id(const uint32_t* pos, uint32_t npos, uint32_t id) {
-  uint32_t lo = 0, hi = npos;
-  while (lo < hi) {
-    const uint32_t mid = (lo + hi) >> 1;
-    if (__ldg(pos + mid) <= id) lo = mid + 1;
-    else hi = mid;
-  }
-  return id + lo;
-}
+// ---- relabel rows (cozo_gpu_hnsw_insert_at, cozo_gpu_hnsw_compact) ------------------------------------------------
+// A monotone map of old row -> new row; NONE drops a row.
 
-// Rows j0 .. j0+rows-1 of one per-node array, staged in `src`, are written to their relabelled rows of `dst`: one warp
-// per row when a row has at least 32 elements, one thread per row otherwise.
-template <class T>
-__global__ void __launch_bounds__(256) shift_rows_kernel(const T* src, T* dst, uint32_t row_elems, uint32_t j0,
-                                                         uint32_t rows, const uint32_t* pos, uint32_t npos) {
+// insert_at: pos holds the ascending insert positions.  Old id j becomes j + #{i : pos[i] <= j}.
+struct GapMap {
+  const uint32_t* pos;
+  uint32_t npos;
+  __device__ __forceinline__ uint32_t operator()(uint32_t id) const {
+    uint32_t lo = 0, hi = npos;
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (__ldg(pos + mid) <= id) lo = mid + 1;
+      else hi = mid;
+    }
+    return id + lo;
+  }
+};
+
+// compact: a table of the new rows, NONE for a dropped row
+struct TableMap {
+  const uint32_t* map;
+  __device__ __forceinline__ uint32_t operator()(uint32_t id) const { return map[id]; }
+};
+
+// Rows j0 .. j0+rows-1 of one array, staged in `src`, are written to rows map(j) of `dst`; dropped rows are not written.
+// One warp per row when a row has at least 32 elements, one thread per row otherwise.
+template <class T, class Map>
+__global__ void __launch_bounds__(256) move_rows_kernel(const T* src, T* dst, uint32_t row_elems, uint32_t j0,
+                                                        uint32_t rows, Map map) {
   const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const bool per_warp = row_elems >= 32;
   const size_t r = per_warp ? t >> 5 : t;
   if (r >= rows) return;
-  const size_t to = relabel_id(pos, npos, j0 + (uint32_t)r);
+  const uint32_t to = map(j0 + (uint32_t)r);
+  if (to == NONE) return;
   for (uint32_t c = per_warp ? (uint32_t)(t & 31) : 0; c < row_elems; c += per_warp ? 32 : 1)
-    dst[to * row_elems + c] = src[(size_t)r * row_elems + c];
+    dst[(size_t)to * row_elems + c] = src[(size_t)r * row_elems + c];
 }
 
-// every stored id (adjacency entries, upper-row owners) through the relabelling; NONE stays NONE
-__global__ void relabel_ids_kernel(uint32_t* ids, size_t count, const uint32_t* pos, uint32_t npos) {
+// every stored id (adjacency entries, upper-row owners, upper_off) through the map; NONE stays NONE.  An id that maps
+// to NONE names a dropped row that a kept row still points at: counted in *bad (hnsw_remove leaves none).
+template <class Map>
+__global__ void map_ids_kernel(uint32_t* ids, size_t count, Map map, uint32_t* bad) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
   const uint32_t v = ids[i];
-  if (v != NONE) ids[i] = relabel_id(pos, npos, v);
+  if (v == NONE) return;
+  const uint32_t to = map(v);
+  if (to == NONE) atomicAdd(bad, 1u);
+  ids[i] = to;
 }
 
 // The rows of the new ids, one warp each: the vector (zero-padded to ld), an empty layer-0 row, level, first upper row,
@@ -634,36 +652,7 @@ __global__ void place_new_rows_kernel(const uint32_t* new_ids, uint32_t count, c
   }
 }
 
-// ---- drop removed ids (cozo_gpu_hnsw_compact) -------------------------------------------------------------------
-// map: old row -> new row, NONE for a dropped row; monotone, never above the old row.
-
-// Forward twin of shift_rows_kernel: rows j0 .. j0+rows-1, staged in `src`, are written to rows map[j] of `dst`;
-// dropped rows are not written.
-template <class T>
-__global__ void __launch_bounds__(256) compact_rows_kernel(const T* src, T* dst, uint32_t row_elems, uint32_t j0,
-                                                           uint32_t rows, const uint32_t* map) {
-  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const bool per_warp = row_elems >= 32;
-  const size_t r = per_warp ? t >> 5 : t;
-  if (r >= rows) return;
-  const uint32_t to = map[j0 + r];
-  if (to == NONE) return;
-  for (uint32_t c = per_warp ? (uint32_t)(t & 31) : 0; c < row_elems; c += per_warp ? 32 : 1)
-    dst[(size_t)to * row_elems + c] = src[(size_t)r * row_elems + c];
-}
-
-// every stored id of a kept row through `map`; NONE stays NONE.  An id that maps to NONE names a dropped row that a
-// kept row still points at: counted in *bad (hnsw_remove leaves none).
-__global__ void compact_ids_kernel(uint32_t* ids, size_t count, const uint32_t* map, uint32_t* bad) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  const uint32_t v = ids[i];
-  if (v == NONE) return;
-  const uint32_t to = map[v];
-  if (to == NONE) atomicAdd(bad, 1u);
-  ids[i] = to;
-}
-
+// ---- the upper-row map of cozo_gpu_hnsw_compact --------------------------------------------------------------
 // keep[r] = 1 for the upper-layer rows whose owner stays; keep[up_rows] = 0 makes the exclusive sum's last element
 // the number of kept rows
 __global__ void upper_keep_kernel(const uint32_t* owner, uint32_t up_rows, const uint32_t* map, uint32_t* keep) {

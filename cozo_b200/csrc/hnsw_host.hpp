@@ -1,5 +1,6 @@
 // hnsw_host.hpp — host-side state of a staged HNSW index (opaque cozo_gpu_hnsw_t).
 #pragma once
+#include <array>
 #include <condition_variable>
 #include <mutex>
 #include <vector>
@@ -75,6 +76,38 @@ struct cozo_gpu_hnsw {
 };
 
 namespace cozo {
+// One per-row device array of a handle: `row_bytes` per node row [0, n), or per upper-layer row [0, up_rows) when
+// `upper`.  Rows from there up to the capacity are unused and hold `fill` bytes, the state append_nodes expects.
+struct RowArray {
+  void*& ptr;
+  size_t row_bytes;
+  bool upper;
+  uint8_t fill;
+};
+
+// Every row array of an f32 handle.  Two of them keep rules of their own: vec may be borrowed from the caller
+// (vec_owned = false) and is then never written, grown or freed; codes is optional (nullptr when the index has no code
+// rows) and is grown by hnsw_codes_reserve, which drops it rather than failing.  vec64 is not listed: every
+// maintenance call refuses F64 handles.
+constexpr size_t kVecArray = 0, kCodesArray = 1;
+inline std::array<RowArray, 12> row_arrays(cozo_gpu_hnsw* h) {
+  const HnswDev& g = h->dev;
+  const size_t vec = (size_t)g.ld * 4, adj0 = (size_t)g.s0 * 4, up = (size_t)g.su * 4;
+  auto ref = [](auto*& p) -> void*& { return reinterpret_cast<void*&>(p); };
+  return {{{ref(h->d_vec), vec, false, 0},
+           {ref(h->d_codes), g.code_ld, false, 0},
+           {ref(h->d_adj0), adj0, false, 0xFF},
+           {ref(h->d_adj0_dist), adj0, false, 0},
+           {ref(h->d_deg0), 4, false, 0},
+           {ref(h->d_upper_off), 4, false, 0xFF},
+           {ref(h->d_node_level), 1, false, 0},
+           {ref(h->d_dead), 1, false, 0},
+           {ref(h->d_adj_up), up, true, 0xFF},
+           {ref(h->d_adj_up_dist), up, true, 0},
+           {ref(h->d_deg_up), 4, true, 0},
+           {ref(h->d_up_owner), 4, true, 0xFF}}};
+}
+
 struct ScatterDest {
   uint32_t n_dest, slot;
   uint32_t* ids[COZO_GPU_MAX_PEERS];

@@ -25,6 +25,11 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from cozo_b200 import capi  # noqa: E402
 
 
+# the relabel's device work; shift_rows_kernel / relabel_ids_kernel are its kernels in builds before the shared routine,
+# so that one script times both
+RELABEL_KERNELS = ("move_rows_kernel", "map_ids_kernel", "shift_rows_kernel", "relabel_ids_kernel", "Memcpy DtoD")
+
+
 def card():
     q = "name,power.limit,clocks.max.sm"
     r = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True)
@@ -99,7 +104,7 @@ def main():
         g.insert_at(np.zeros(1, np.uint32), V1)
     us = 0.0
     for e in prof.key_averages():
-        if any(k in e.key for k in ("shift_rows_kernel", "relabel_ids_kernel", "Memcpy DtoD")):
+        if any(k in e.key for k in RELABEL_KERNELS):
             us += getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0))
     nb = relabel_bytes(n, n + 1, n // (a.m - 1), a.dim, a.m)
     emit({"what": "c_relabel_device_time", "n": n, "relabel_ms": us / 1e3, "relabel_bytes": nb,

@@ -28,6 +28,12 @@ for dim, metric in [(64, capi.L2), (100, capi.COSINE)]:
     g.remove(np.arange(100, 160, dtype=np.uint32))
     ids3, _, cnt3, _ = g.search(Q, 5, 40)
     assert (cnt3 == 5).all() and not np.isin(ids3, np.arange(100, 160)).any()
+    # rows inside the key range (front, middle, end), then the removed rows dropped: both relabellings
+    for pos in (0, 850, g.info()[0]):
+        g.insert_at(np.full(3, pos, np.uint32), rng.random((3, dim), dtype=np.float32) - 0.5)
+    g.remove(np.arange(400, 420, dtype=np.uint32))
+    g.compact()
+    assert (g.search(Q, 5, 40)[2] == 5).all()
     g.export_levels(); g.export_dists(); g.export_live()
 src = rng.integers(0, 300, 3000).astype(np.uint32)
 dst = rng.integers(0, 300, 3000).astype(np.uint32)
