@@ -31,6 +31,8 @@ EXPORTS = [
     "cozo_gpu_hnsw_stage_sharded", "cozo_gpu_hnsw_search_sharded", "cozo_gpu_hnsw_search_sharded_dev",
     "cozo_gpu_hnsw_search_filtered", "cozo_gpu_hnsw_search_filtered_dev", "cozo_gpu_hnsw_search_f64",
     "cozo_gpu_graph_stage_keys", "cozo_gpu_graph_node_endpoints", "cozo_gpu_graph_lookup_keys",
+    "cozo_gpu_hnsw_search_sharded_filtered", "cozo_gpu_hnsw_search_sharded_filtered_dev",
+    "cozo_gpu_hnsw_search_sharded_f64",
 ]
 UID_BYTES = 128
 
@@ -125,6 +127,11 @@ def load():
     L.cozo_gpu_hnsw_stage_sharded.argtypes = [vp, vp, vp, vp]
     L.cozo_gpu_hnsw_search_sharded.argtypes = [vp, vp, u32, u32, u32, f64, C.c_int, vp, vp, vp, C.POINTER(SearchStats)]
     L.cozo_gpu_hnsw_search_sharded_dev.argtypes = [vp, vp, u32, u32, u32, f64, vp, vp, vp, vp]
+    L.cozo_gpu_hnsw_search_sharded_filtered.argtypes = [vp, vp, u32, u32, u32, f64, C.c_int, vp, vp, vp, vp,
+                                                        C.POINTER(SearchStats)]
+    L.cozo_gpu_hnsw_search_sharded_filtered_dev.argtypes = [vp, vp, u32, u32, u32, f64, vp, vp, vp, vp, vp]
+    L.cozo_gpu_hnsw_search_sharded_f64.argtypes = [vp, vp, u32, u32, u32, f64, C.c_int, vp, vp, vp, vp,
+                                                   C.POINTER(SearchStats)]
     _lib = L
     return L
 
@@ -411,25 +418,48 @@ class ShardGroup:
         _check(load().cozo_gpu_shards_info(self._h, C.byref(r), C.byref(w), C.byref(x), C.byref(t)))
         return {"rank": r.value, "world": w.value, "exchange": "fused" if x.value else "nccl", "total_rows": t.value}
 
-    def search(self, queries, k: int, ef: int, radius: float | None = None, root: int = -1, B: int | None = None):
-        """collective host-buffer call -> global ids[B,k] u64 (UINT64_MAX padded), dist[B,k], count[B], stats"""
+    def _search(self, fn, dtype, queries, k, ef, radius, root, B, row_pass, takes_mask):
         if queries is not None:
-            queries = np.ascontiguousarray(queries, np.float32).reshape(-1, self.index.dim)
+            queries = np.ascontiguousarray(queries, dtype).reshape(-1, self.index.dim)
             B = queries.shape[0]
         ids = np.empty((B, max(k, 1)), np.uint64)
-        dist = np.empty((B, max(k, 1)), np.float32)
+        dist = np.empty((B, max(k, 1)), dtype)
         cnt = np.zeros(B, np.uint32)
         st = SearchStats()
-        _check(load().cozo_gpu_hnsw_search_sharded(self._h, _p(queries), B, k, ef,
-                                                   -1.0 if radius is None else float(radius), root, _p(ids), _p(dist),
-                                                   _p(cnt), C.byref(st)))
+        mask = None if row_pass is None else pack_row_mask(row_pass)
+        args = (_p(mask),) if takes_mask else ()
+        _check(fn(self._h, _p(queries), B, k, ef, -1.0 if radius is None else float(radius), root, *args, _p(ids),
+                  _p(dist), _p(cnt), C.byref(st)))
         return ids, dist, cnt, st
 
+    def search(self, queries, k: int, ef: int, radius: float | None = None, root: int = -1, B: int | None = None,
+               row_pass=None):
+        """collective host-buffer call -> global ids[B,k] u64 (UINT64_MAX padded), dist[B,k], count[B], stats.
+        row_pass: optional bool[n_local] filter verdicts over this rank's rows (the filtered form)"""
+        L = load()
+        if row_pass is None:
+            return self._search(L.cozo_gpu_hnsw_search_sharded, np.float32, queries, k, ef, radius, root, B, None,
+                                False)
+        return self._search(L.cozo_gpu_hnsw_search_sharded_filtered, np.float32, queries, k, ef, radius, root, B,
+                            row_pass, True)
+
+    def search_f64(self, queries, k: int, ef: int, radius: float | None = None, root: int = -1, B: int | None = None,
+                   row_pass=None):
+        """collective host-buffer call on a group of F64 shards -> global ids[B,k] u64, dist[B,k] f64, count[B], stats"""
+        return self._search(load().cozo_gpu_hnsw_search_sharded_f64, np.float64, queries, k, ef, radius, root, B,
+                            row_pass, True)
+
     def search_dev(self, q_ptr: int, B: int, k: int, ef: int, out_ids_ptr: int, out_dist_ptr: int,
-                   qstats_ptr: int | None = None, stream: int | None = None, radius: float | None = None):
-        _check(load().cozo_gpu_hnsw_search_sharded_dev(self._h, q_ptr, B, k, ef,
-                                                       -1.0 if radius is None else float(radius), out_ids_ptr,
-                                                       out_dist_ptr, qstats_ptr, stream))
+                   qstats_ptr: int | None = None, stream: int | None = None, radius: float | None = None,
+                   row_mask_ptr: int | None = None):
+        """row_mask_ptr: device pointer of this rank's packed verdicts (pack_row_mask layout), the filtered form"""
+        r = -1.0 if radius is None else float(radius)
+        if row_mask_ptr is None:
+            _check(load().cozo_gpu_hnsw_search_sharded_dev(self._h, q_ptr, B, k, ef, r, out_ids_ptr, out_dist_ptr,
+                                                           qstats_ptr, stream))
+        else:
+            _check(load().cozo_gpu_hnsw_search_sharded_filtered_dev(self._h, q_ptr, B, k, ef, r, row_mask_ptr,
+                                                                    out_ids_ptr, out_dist_ptr, qstats_ptr, stream))
 
     def close(self):
         if self._h:

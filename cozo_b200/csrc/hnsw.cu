@@ -843,10 +843,10 @@ static int check_search_args(cozo_gpu_hnsw_t* h, uint32_t k, uint32_t ef) {
   return 0;
 }
 
-static int search_dev_impl(cozo_gpu_hnsw_t* h, const float* queries_dev, uint32_t B, uint32_t k, uint32_t ef,
-                           double radius, uint32_t* out_ids_dev, float* out_dist_dev, uint32_t* out_count_dev,
-                           uint32_t* per_query_stats_dev, void* stream, const ScatterDest* scatter,
-                           const uint32_t* filter_mask_dev = nullptr) {
+int cozo::hnsw_search_dev(cozo_gpu_hnsw_t* h, const float* queries_dev, uint32_t B, uint32_t k, uint32_t ef,
+                          double radius, uint32_t* out_ids_dev, float* out_dist_dev, uint32_t* out_count_dev,
+                          uint32_t* per_query_stats_dev, void* stream, const ScatterDest* scatter,
+                          const uint32_t* filter_mask_dev) {
   int rc = check_search_args(h, k, ef);
   if (rc) return rc;
   if (B && !queries_dev) return set_error(COZO_GPU_EINVAL, "null buffer");
@@ -888,8 +888,8 @@ static int search_dev_impl(cozo_gpu_hnsw_t* h, const float* queries_dev, uint32_
 extern "C" int cozo_gpu_hnsw_search_dev(cozo_gpu_hnsw_t* h, const float* queries_dev, uint32_t B, uint32_t k,
                                         uint32_t ef, double radius, uint32_t* out_ids_dev, float* out_dist_dev,
                                         uint32_t* out_count_dev, uint32_t* per_query_stats_dev, void* stream) {
-  return search_dev_impl(h, queries_dev, B, k, ef, radius, out_ids_dev, out_dist_dev, out_count_dev,
-                         per_query_stats_dev, stream, nullptr);
+  return hnsw_search_dev(h, queries_dev, B, k, ef, radius, out_ids_dev, out_dist_dev, out_count_dev,
+                         per_query_stats_dev, stream, nullptr, nullptr);
 }
 
 extern "C" int cozo_gpu_hnsw_search_scatter_dev(cozo_gpu_hnsw_t* h, const float* queries_dev, uint32_t B, uint32_t k,
@@ -906,7 +906,8 @@ extern "C" int cozo_gpu_hnsw_search_scatter_dev(cozo_gpu_hnsw_t* h, const float*
     sc.dist[d] = reinterpret_cast<float*>(dest_dist_ptrs[d]);
     if (!sc.ids[d] || !sc.dist[d]) return set_error(COZO_GPU_EINVAL, "null destination buffer");
   }
-  return search_dev_impl(h, queries_dev, B, k, ef, radius, nullptr, nullptr, nullptr, per_query_stats_dev, stream, &sc);
+  return hnsw_search_dev(h, queries_dev, B, k, ef, radius, nullptr, nullptr, nullptr, per_query_stats_dev, stream, &sc,
+                         nullptr);
 }
 
 static int search_host_impl(cozo_gpu_hnsw_t* h, const float* queries, uint32_t B, uint32_t k, uint32_t ef, double radius,
@@ -1017,7 +1018,7 @@ extern "C" int cozo_gpu_hnsw_search_filtered_dev(cozo_gpu_hnsw_t* h, const float
                                                  uint32_t* out_ids_dev, float* out_dist_dev, uint32_t* out_count_dev,
                                                  uint32_t* per_query_stats_dev, void* stream) {
   if (!row_mask_dev) return set_error(COZO_GPU_EINVAL, "null row mask");
-  return search_dev_impl(h, queries_dev, B, k, ef, radius, out_ids_dev, out_dist_dev, out_count_dev,
+  return hnsw_search_dev(h, queries_dev, B, k, ef, radius, out_ids_dev, out_dist_dev, out_count_dev,
                          per_query_stats_dev, stream, nullptr, row_mask_dev);
 }
 

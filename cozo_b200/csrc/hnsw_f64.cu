@@ -32,6 +32,11 @@ struct Search64Params {
   uint32_t logcap;
   uint32_t warp_smem, off_fi, off_pend, off_q;
   const uint32_t* filter_mask;
+  // fused exchange of the sharded corpus, as in SearchParams: besides (or instead of) out_ids/out_dist the top-k of
+  // query qi is stored into every destination's [n_slots][B][k] gather buffer at slot `slot`
+  uint32_t n_dest, slot;
+  uint32_t* dest_ids[COZO_GPU_MAX_PEERS];
+  double* dest_dist[COZO_GPU_MAX_PEERS];
 };
 
 __device__ __forceinline__ double warp_sum_f64(double v) {
@@ -159,6 +164,18 @@ __device__ __forceinline__ void search_level64(const HnswDev& g, const Search64P
   visit_clear(w, lane);
 }
 
+// result i of query qi: into out_ids/out_dist, and into every destination's gather buffer.  out_ids/out_dist are
+// always written: testing them for null next to the destination loop makes ptxas spill.
+__device__ __forceinline__ void store64(const Search64Params& p, uint32_t qi, uint32_t i, uint32_t oid, double od) {
+  p.out_ids[(size_t)qi * p.k + i] = oid;
+  p.out_dist[(size_t)qi * p.k + i] = od;
+  const size_t at = ((size_t)p.slot * p.B + qi) * p.k + i;
+  for (uint32_t d = 0; d < p.n_dest; ++d) {  // the all-gather, fused into the epilogue
+    p.dest_ids[d][at] = oid;
+    p.dest_dist[d][at] = od;
+  }
+}
+
 template <int METRIC>
 __global__ void __launch_bounds__(128) hnsw_search_f64_kernel(HnswDev g, Search64Params p) {
   extern __shared__ __align__(16) uint8_t smem64[];
@@ -226,18 +243,12 @@ __global__ void __launch_bounds__(128) hnsw_search_f64_kernel(HnswDev g, Search6
         }
         const uint32_t bal = __ballot_sync(0xffffffffu, ok);
         const uint32_t pos = found + __popc(bal & ((1u << lane) - 1));
-        if (ok && pos < p.k) {
-          p.out_ids[(size_t)qi * p.k + pos] = id;
-          p.out_dist[(size_t)qi * p.k + pos] = d2;
-        }
+        if (ok && pos < p.k) store64(p, qi, pos, id, d2);
         found += __popc(bal);
       }
       if (found > p.k) found = p.k;
     }
-    for (uint32_t i = found + lane; i < p.k; i += 32) {
-      p.out_ids[(size_t)qi * p.k + i] = NONE;
-      p.out_dist[(size_t)qi * p.k + i] = INFINITY;
-    }
+    for (uint32_t i = found + lane; i < p.k; i += 32) store64(p, qi, i, NONE, INFINITY);
     if (lane == 0) {
       if (p.out_count) p.out_count[qi] = found;
       if (p.qstats) reinterpret_cast<uint4*>(p.qstats)[qi] = make_uint4(w.dist_evals, w.nodes_expanded, w.nbr_reads, 0);
@@ -248,35 +259,12 @@ __global__ void __launch_bounds__(128) hnsw_search_f64_kernel(HnswDev g, Search6
 
 }  // namespace cozo
 
-using namespace cozo;
-
-extern "C" int cozo_gpu_hnsw_search_f64(cozo_gpu_hnsw_t* h, const double* queries, uint32_t B, uint32_t k, uint32_t ef,
-                                        double radius, const uint32_t* row_mask, uint32_t* out_ids, double* out_dist,
-                                        uint32_t* out_count, CozoGpuSearchStats* stats) {
-  if (!h) return set_error(COZO_GPU_EINVAL, "null index handle");
-  if (!h->f64) return set_error(COZO_GPU_EINVAL, "not an F64 index: use cozo_gpu_hnsw_search");
-  if (k == 0) return set_error(COZO_GPU_EINVAL, "k must be positive");
-  if (ef == 0) return set_error(COZO_GPU_EINVAL, "ef must be positive");
-  if (B && (!queries || !out_ids || !out_dist)) return set_error(COZO_GPU_EINVAL, "null buffer");
-  int rc = ensure_init();
-  if (rc) return rc;
-  if (stats) memset(stats, 0, sizeof(*stats));
-  if (B == 0) return 0;
+int cozo::hnsw_launch_search_f64(cozo_gpu_hnsw* h, HnswWorkspace* ws, const double* d_q, uint32_t B, uint32_t k,
+                                  uint32_t ef, double radius, uint32_t* d_ids, double* d_dist, uint32_t* d_count,
+                                  uint32_t* d_qstats, cudaStream_t st, const ScatterDest64* scatter,
+                                  const uint32_t* d_filter_mask) {
   const DeviceInfo& di = device_info();
   const HnswDev& g = h->dev;
-  HnswWorkspace* ws = hnsw_acquire_ws(h);
-  if (!ws) return COZO_GPU_ECUDA;
-  struct Bufs {
-    cozo_gpu_hnsw* h;
-    HnswWorkspace* ws;
-    void* p[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    ~Bufs() {
-      for (void* q : p)
-        if (q) cudaFree(q);
-      hnsw_release_ws(h, ws);
-    }
-  } bf{h, ws};
-  cudaStream_t st = ws->stream;
   Search64Params p{};
   const uint32_t efcap = round_up(ef, 32);
   p.off_fi = efcap * 8;
@@ -304,8 +292,68 @@ extern "C" int cozo_gpu_hnsw_search_f64(cozo_gpu_hnsw_t* h, const double* querie
   const uint32_t nwords = round_up((g.n + 31) / 32, 4);
   const uint32_t logcap = std::min<uint32_t>(65536u, std::max<uint32_t>(4096u, 64u * ef));
   const size_t slots = (size_t)grid * wpc;
-  rc = hnsw_ws_reserve(ws, slots * nwords, slots * logcap, st);
+  int rc = hnsw_ws_reserve(ws, slots * nwords, slots * logcap, st);
   if (rc) return rc;
+  p.queries = d_q;
+  p.vec64 = h->d_vec64;
+  p.ld64 = h->ld64;
+  p.B = B;
+  p.k = k;
+  p.ef = ef;
+  p.has_radius = radius >= 0.0;
+  p.radius = radius;
+  p.out_ids = d_ids;
+  p.out_dist = d_dist;
+  p.out_count = d_count;
+  p.qstats = d_qstats;
+  p.counter = ws->counter;
+  p.vis = ws->vis;
+  p.nwords = nwords;
+  p.vlog = ws->vlog;
+  p.logcap = logcap;
+  p.filter_mask = d_filter_mask;
+  if (scatter) {
+    p.n_dest = scatter->n_dest;
+    p.slot = scatter->slot;
+    for (uint32_t d = 0; d < scatter->n_dest; ++d) {
+      p.dest_ids[d] = scatter->ids[d];
+      p.dest_dist[d] = scatter->dist[d];
+    }
+  }
+  COZO_CUDA(cudaMemsetAsync(ws->counter, 0, 4, st));
+  fn<<<grid, wpc * 32, smem, st>>>(g, p);
+  COZO_CUDA(cudaGetLastError());
+  return 0;
+}
+
+using namespace cozo;
+
+extern "C" int cozo_gpu_hnsw_search_f64(cozo_gpu_hnsw_t* h, const double* queries, uint32_t B, uint32_t k, uint32_t ef,
+                                        double radius, const uint32_t* row_mask, uint32_t* out_ids, double* out_dist,
+                                        uint32_t* out_count, CozoGpuSearchStats* stats) {
+  if (!h) return set_error(COZO_GPU_EINVAL, "null index handle");
+  if (!h->f64) return set_error(COZO_GPU_EINVAL, "not an F64 index: use cozo_gpu_hnsw_search");
+  if (k == 0) return set_error(COZO_GPU_EINVAL, "k must be positive");
+  if (ef == 0) return set_error(COZO_GPU_EINVAL, "ef must be positive");
+  if (B && (!queries || !out_ids || !out_dist)) return set_error(COZO_GPU_EINVAL, "null buffer");
+  int rc = ensure_init();
+  if (rc) return rc;
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (B == 0) return 0;
+  const HnswDev& g = h->dev;
+  HnswWorkspace* ws = hnsw_acquire_ws(h);
+  if (!ws) return COZO_GPU_ECUDA;
+  struct Bufs {
+    cozo_gpu_hnsw* h;
+    HnswWorkspace* ws;
+    void* p[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    ~Bufs() {
+      for (void* q : p)
+        if (q) cudaFree(q);
+      hnsw_release_ws(h, ws);
+    }
+  } bf{h, ws};
+  cudaStream_t st = ws->stream;
   const size_t qb = (size_t)B * g.dim * 8;
   COZO_CUDA(cudaMalloc(&bf.p[0], qb));
   COZO_CUDA(cudaMalloc(&bf.p[1], (size_t)B * k * 4));
@@ -318,28 +366,12 @@ extern "C" int cozo_gpu_hnsw_search_f64(cozo_gpu_hnsw_t* h, const double* querie
     COZO_CUDA(cudaMemcpyAsync(bf.p[5], row_mask, words * 4, cudaMemcpyHostToDevice, st));
   }
   COZO_CUDA(cudaMemcpyAsync(bf.p[0], queries, qb, cudaMemcpyHostToDevice, st));
-  p.queries = static_cast<const double*>(bf.p[0]);
-  p.vec64 = h->d_vec64;
-  p.ld64 = h->ld64;
-  p.B = B;
-  p.k = k;
-  p.ef = ef;
-  p.has_radius = radius >= 0.0;
-  p.radius = radius;
-  p.out_ids = static_cast<uint32_t*>(bf.p[1]);
-  p.out_dist = static_cast<double*>(bf.p[2]);
-  p.out_count = static_cast<uint32_t*>(bf.p[3]);
-  p.qstats = static_cast<uint32_t*>(bf.p[4]);
-  p.counter = ws->counter;
-  p.vis = ws->vis;
-  p.nwords = nwords;
-  p.vlog = ws->vlog;
-  p.logcap = logcap;
-  p.filter_mask = row_mask ? static_cast<const uint32_t*>(bf.p[5]) : nullptr;
-  COZO_CUDA(cudaMemsetAsync(ws->counter, 0, 4, st));
   COZO_CUDA(cudaEventRecord(ws->e0, st));
-  fn<<<grid, wpc * 32, smem, st>>>(g, p);
-  COZO_CUDA(cudaGetLastError());
+  rc = hnsw_launch_search_f64(h, ws, static_cast<const double*>(bf.p[0]), B, k, ef, radius,
+                              static_cast<uint32_t*>(bf.p[1]), static_cast<double*>(bf.p[2]),
+                              static_cast<uint32_t*>(bf.p[3]), static_cast<uint32_t*>(bf.p[4]), st, nullptr,
+                              row_mask ? static_cast<const uint32_t*>(bf.p[5]) : nullptr);
+  if (rc) return rc;
   COZO_CUDA(cudaEventRecord(ws->e1, st));
   COZO_CUDA(cudaMemcpyAsync(out_ids, bf.p[1], (size_t)B * k * 4, cudaMemcpyDeviceToHost, st));
   COZO_CUDA(cudaMemcpyAsync(out_dist, bf.p[2], (size_t)B * k * 8, cudaMemcpyDeviceToHost, st));

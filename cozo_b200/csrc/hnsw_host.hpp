@@ -108,14 +108,31 @@ inline std::array<RowArray, 12> row_arrays(cozo_gpu_hnsw* h) {
            {ref(h->d_up_owner), 4, true, 0xFF}}};
 }
 
-struct ScatterDest {
+// destinations of the fused exchange: the [n_slots][B][k] gather buffers of every rank, this rank's lists at `slot`
+template <typename D>
+struct ScatterDestT {
   uint32_t n_dest, slot;
   uint32_t* ids[COZO_GPU_MAX_PEERS];
-  float* dist[COZO_GPU_MAX_PEERS];
+  D* dist[COZO_GPU_MAX_PEERS];
 };
+using ScatterDest = ScatterDestT<float>;
+using ScatterDest64 = ScatterDestT<double>;
 int hnsw_launch_search(cozo_gpu_hnsw* h, HnswWorkspace* ws, const float* d_q, uint32_t B, uint32_t k, uint32_t ef,
                        double radius, uint32_t* d_ids, float* d_dist, uint32_t* d_count, uint32_t* d_qstats,
                        cudaStream_t stream, const ScatterDest* scatter, const uint32_t* d_filter_mask = nullptr);
+// the asynchronous f32 search of cozo_gpu_hnsw_search_dev / _filtered_dev / _scatter_dev: checks the arguments, takes
+// a workspace and hands it back after the kernel, in stream order
+int hnsw_search_dev(cozo_gpu_hnsw* h, const float* d_q, uint32_t B, uint32_t k, uint32_t ef, double radius,
+                    uint32_t* d_ids, float* d_dist, uint32_t* d_count, uint32_t* d_qstats, void* stream,
+                    const ScatterDest* scatter, const uint32_t* d_filter_mask);
+// the F64 search kernel on device buffers, on `stream`, with `ws` held by the caller until the kernel ends.  d_ids /
+// d_dist [B*k] are always written, also when `scatter` is given; d_count, d_qstats, scatter and d_filter_mask nullable.
+int hnsw_launch_search_f64(cozo_gpu_hnsw* h, HnswWorkspace* ws, const double* d_q, uint32_t B, uint32_t k, uint32_t ef,
+                           double radius, uint32_t* d_ids, double* d_dist, uint32_t* d_count, uint32_t* d_qstats,
+                           cudaStream_t stream, const ScatterDest64* scatter, const uint32_t* d_filter_mask);
+// merge.cu: cozo_gpu_topk_merge_dev on F64 distances
+int topk_merge_f64_dev(const double* dist_dev, const uint32_t* ids_dev, uint32_t n_shards, uint32_t B, uint32_t k,
+                       const uint64_t* shard_offsets_dev, uint64_t* out_ids_dev, double* out_dist_dev, void* stream);
 HnswWorkspace* hnsw_acquire_ws(cozo_gpu_hnsw* h);
 void hnsw_release_ws(cozo_gpu_hnsw* h, HnswWorkspace* ws);
 int hnsw_ws_reserve(HnswWorkspace* ws, size_t vis_words, size_t vlog_words, cudaStream_t stream);

@@ -19,6 +19,7 @@
 #include <algorithm>
 #include <cstring>
 #include <mutex>
+#include <type_traits>
 #include <vector>
 
 #include "hnsw_host.hpp"
@@ -87,31 +88,34 @@ struct cozo_gpu_shards {
   cozo_gpu_hnsw* shard = nullptr;
   std::vector<uint64_t> offsets;  // global id of every shard's row 0 (row-contiguous partition)
   uint64_t total_rows = 0;
+  int dtype = 0;  // every shard's VecElementType, agreed at attach: 0 = F32, 1 = F64, -1 = the shards mix them
   uint64_t* d_offsets = nullptr;
   cudaStream_t stream = nullptr;
   int exchange = 0;  // 0 = NCCL all-gather, 1 = fused peer stores
   std::string fused_why_not;
-  // capacity of the exchange buffers: `tile` queries of `k` results
-  uint32_t tile_cap = 0, k_cap = 0;
-  // one IPC-shareable block per rank: [flags 256 B][set 0: ids S*tile*k, dist S*tile*k][set 1: ...]
+  // capacity of the exchange buffers: `tile` queries of `k` results, distances of `dsz_cap` bytes (4 or 8)
+  uint32_t tile_cap = 0, k_cap = 0, dsz_cap = 0;
+  // one IPC-shareable block per rank: [flags 256 B][set 0: ids S*tile*k u32, dist S*tile*k][set 1: ...]
   uint8_t* block = nullptr;
   size_t block_bytes = 0;
   uint8_t* peer_block[COZO_GPU_MAX_PEERS] = {};  // this rank's view of every rank's block (self = block)
   uint32_t* local_ids[2] = {nullptr, nullptr};   // NCCL form: the all-gather's send buffers
-  float* local_dist[2] = {nullptr, nullptr};
+  void* local_dist[2] = {nullptr, nullptr};
   uint32_t epoch = 0;
   // running tile counter: consecutive tiles — of one call or of consecutive calls — alternate between the two
   // buffer sets.  A rank may only overwrite a peer's set once that peer has merged what the set held; passing the
   // barrier of tile i proves every peer has finished merging tile i-1 (stream order on the peer), i.e. the OTHER set.
   uint32_t tile_seq = 0;
   int* d_timeout = nullptr;
-  // staging of the host-pointer call
-  float* d_q = nullptr;
-  size_t q_floats = 0;
+  // staging of the host-pointer calls (f32 or f64 queries; distances sized for f64)
+  void* d_q = nullptr;
+  size_t q_bytes = 0;
   uint64_t* d_out_ids = nullptr;
-  float* d_out_dist = nullptr;
+  void* d_out_dist = nullptr;
   uint32_t* d_qstats = nullptr;
   size_t out_rows = 0, out_k = 0;
+  uint32_t* d_mask = nullptr;  // row filter verdicts of the host-pointer call, uploaded once per call
+  size_t mask_words = 0;
   std::mutex mu;  // one sharded search at a time per communicator (collectives must not interleave)
 };
 
@@ -143,15 +147,19 @@ __global__ void shard_barrier_kernel(uint32_t* my_flags, PeerFlagPtrs peers, int
   }
 }
 
-static size_t set_bytes(const cozo_gpu_shards* s, uint32_t tile, uint32_t k) {
-  return (size_t)s->world * tile * k * 4;  // one list (ids or dist) of one set
+static size_t ids_bytes(const cozo_gpu_shards* s, uint32_t tile, uint32_t k) {
+  // the id list of one set, padded so that the distances after it stay aligned for f64
+  return ((size_t)s->world * tile * k * 4 + 255) & ~(size_t)255;
+}
+static size_t set_bytes(const cozo_gpu_shards* s, uint32_t tile, uint32_t k, uint32_t dsz) {
+  return ids_bytes(s, tile, k) * (1 + dsz / 4);  // ids, then distances of dsz bytes
 }
 static uint32_t* set_ids(uint8_t* blk, const cozo_gpu_shards* s, int b) {
-  return reinterpret_cast<uint32_t*>(blk + 256 + (size_t)b * 2 * set_bytes(s, s->tile_cap, s->k_cap));
+  return reinterpret_cast<uint32_t*>(blk + 256 + (size_t)b * set_bytes(s, s->tile_cap, s->k_cap, s->dsz_cap));
 }
-static float* set_dist(uint8_t* blk, const cozo_gpu_shards* s, int b) {
-  return reinterpret_cast<float*>(blk + 256 + (size_t)b * 2 * set_bytes(s, s->tile_cap, s->k_cap) +
-                                  set_bytes(s, s->tile_cap, s->k_cap));
+template <typename D>
+static D* set_dist(uint8_t* blk, const cozo_gpu_shards* s, int b) {
+  return reinterpret_cast<D*>(reinterpret_cast<uint8_t*>(set_ids(blk, s, b)) + ids_bytes(s, s->tile_cap, s->k_cap));
 }
 
 static void close_peers(cozo_gpu_shards* s) {
@@ -161,13 +169,14 @@ static void close_peers(cozo_gpu_shards* s) {
   }
 }
 
-// (Re)allocate the exchange buffers for `tile` x `k` and, for the fused form, open every peer's block.
-// Collective: all ranks call it with the same arguments.
-static int ensure_exchange(cozo_gpu_shards* s, uint32_t tile, uint32_t k) {
-  if (tile <= s->tile_cap && k <= s->k_cap && s->block) return 0;
+// (Re)allocate the exchange buffers for `tile` x `k` distances of `dsz` bytes and, for the fused form, open every peer's
+// block.  Collective: all ranks call it with the same arguments.
+static int ensure_exchange(cozo_gpu_shards* s, uint32_t tile, uint32_t k, uint32_t dsz) {
+  if (tile <= s->tile_cap && k <= s->k_cap && dsz <= s->dsz_cap && s->block) return 0;
   COZO_CUDA(cudaStreamSynchronize(s->stream));
   tile = std::max(tile, s->tile_cap);
   k = std::max(k, s->k_cap);
+  dsz = std::max(dsz, s->dsz_cap);
   close_peers(s);
   if (s->block && s->world > 1) {
     // every rank has closed its mappings of the old blocks before any rank frees one (freeing exported memory
@@ -188,14 +197,15 @@ static int ensure_exchange(cozo_gpu_shards* s, uint32_t tile, uint32_t k) {
   }
   s->tile_cap = tile;
   s->k_cap = k;
-  s->block_bytes = 256 + 4 * set_bytes(s, tile, k);
+  s->dsz_cap = dsz;
+  s->block_bytes = 256 + 2 * set_bytes(s, tile, k, dsz);
   COZO_CUDA(cudaMalloc(&s->block, s->block_bytes));
   COZO_CUDA(cudaMemsetAsync(s->block, 0, 256, s->stream));  // ordered before the handle exchange below
   s->epoch = 0;
   s->tile_seq = 0;
   for (int b = 0; b < 2; ++b) {
     COZO_CUDA(cudaMalloc(&s->local_ids[b], (size_t)tile * k * 4));
-    COZO_CUDA(cudaMalloc(&s->local_dist[b], (size_t)tile * k * 4));
+    COZO_CUDA(cudaMalloc(&s->local_dist[b], (size_t)tile * k * dsz));
   }
   s->peer_block[s->rank] = s->block;
   if (s->world == 1) {
@@ -260,31 +270,48 @@ static int ensure_exchange(cozo_gpu_shards* s, uint32_t tile, uint32_t k) {
   return 0;
 }
 
-// the device form: everything already in HBM, asynchronous on the communicator's stream
-static int sharded_search_dev(cozo_gpu_shards* s, const float* d_q, uint32_t B, uint32_t k, uint32_t ef, double radius,
-                              uint64_t* d_out_ids, float* d_out_dist, uint32_t* d_qstats) {
+// the device form: everything already in HBM, asynchronous on the communicator's stream.  T is the distance (and
+// query) type of the group; d_mask = this rank's filter verdicts (nullptr = no filter).  F64 groups search with `ws64`,
+// a workspace of the shard the caller holds until the stream has drained.
+template <typename T>
+static int sharded_search_dev(cozo_gpu_shards* s, const T* d_q, uint32_t B, uint32_t k, uint32_t ef, double radius,
+                              const uint32_t* d_mask, uint64_t* d_out_ids, T* d_out_dist, uint32_t* d_qstats,
+                              HnswWorkspace* ws64 = nullptr) {
+  constexpr bool f64 = std::is_same<T, double>::value;
   cozo_gpu_hnsw* h = s->shard;
   const uint32_t dim = h->dev.dim;
   uint32_t tile = (uint32_t)std::max<int64_t>(1, get_option("shard.tile", 65536));
   tile = std::min(tile, std::max(B, 1u));
-  int rc = ensure_exchange(s, tile, k);
+  int rc = ensure_exchange(s, tile, k, sizeof(T));
   if (rc) return rc;
   cudaStream_t st = s->stream;
   for (uint32_t q0 = 0; q0 < B; q0 += tile) {
     const uint32_t nq = std::min(tile, B - q0);
     const int b = (int)(s->tile_seq++ & 1u);  // NOT the tile index of this call: back-to-back single-tile calls must alternate too
-    const float* q = d_q + (size_t)q0 * dim;
+    const T* q = d_q + (size_t)q0 * dim;
     uint32_t* qs = d_qstats ? d_qstats + (size_t)q0 * 4 : nullptr;
+    T* local_dist = static_cast<T*>(s->local_dist[b]);
+    // fused: the gather layout of this tile, [world][nq][k] at the start of set b of every rank
+    ScatterDestT<T> sc{};
+    const ScatterDestT<T>* scatter = nullptr;
     if (s->exchange == 1) {
-      // gather layout of this tile: [world][nq][k] at the start of set b
-      uint64_t dids[COZO_GPU_MAX_PEERS], ddist[COZO_GPU_MAX_PEERS];
+      sc.n_dest = (uint32_t)s->world;
+      sc.slot = (uint32_t)s->rank;
       for (int r = 0; r < s->world; ++r) {
-        dids[r] = reinterpret_cast<uint64_t>(set_ids(s->peer_block[r], s, b));
-        ddist[r] = reinterpret_cast<uint64_t>(set_dist(s->peer_block[r], s, b));
+        sc.ids[r] = set_ids(s->peer_block[r], s, b);
+        sc.dist[r] = set_dist<T>(s->peer_block[r], s, b);
       }
-      rc = cozo_gpu_hnsw_search_scatter_dev(h, q, nq, k, ef, radius, (uint32_t)s->world, dids, ddist, (uint32_t)s->rank,
-                                            qs, st);
-      if (rc) return rc;
+      scatter = &sc;
+    }
+    if constexpr (f64)  // the kernel also writes the local lists: the NCCL form sends them
+      rc = hnsw_launch_search_f64(h, ws64, q, nq, k, ef, radius, s->local_ids[b], local_dist, nullptr, qs, st, scatter,
+                                  d_mask);
+    else if (scatter)
+      rc = hnsw_search_dev(h, q, nq, k, ef, radius, nullptr, nullptr, nullptr, qs, st, scatter, d_mask);
+    else
+      rc = hnsw_search_dev(h, q, nq, k, ef, radius, s->local_ids[b], local_dist, nullptr, qs, st, nullptr, d_mask);
+    if (rc) return rc;
+    if (s->exchange == 1) {
       if (s->world > 1) {
         PeerFlagPtrs pf{};
         for (int r = 0; r < s->world; ++r) pf.p[r] = reinterpret_cast<uint32_t*>(s->peer_block[r]);
@@ -293,23 +320,37 @@ static int sharded_search_dev(cozo_gpu_shards* s, const float* d_q, uint32_t B, 
                                                s->d_timeout);
         COZO_CUDA(cudaGetLastError());
       }
+    } else if (s->world > 1) {
+      COZO_NCCL(g_nccl.GroupStart());
+      COZO_NCCL(g_nccl.AllGather(s->local_ids[b], set_ids(s->block, s, b), (size_t)nq * k, ncclUint32, s->comm, st));
+      COZO_NCCL(g_nccl.AllGather(local_dist, set_dist<T>(s->block, s, b), (size_t)nq * k, f64 ? ncclFloat64 : ncclFloat32,
+                                 s->comm, st));
+      COZO_NCCL(g_nccl.GroupEnd());
     } else {
-      rc = cozo_gpu_hnsw_search_dev(h, q, nq, k, ef, radius, s->local_ids[b], s->local_dist[b], nullptr, qs, st);
-      if (rc) return rc;
-      if (s->world > 1) {
-        COZO_NCCL(g_nccl.GroupStart());
-        COZO_NCCL(g_nccl.AllGather(s->local_ids[b], set_ids(s->block, s, b), (size_t)nq * k, ncclUint32, s->comm, st));
-        COZO_NCCL(g_nccl.AllGather(s->local_dist[b], set_dist(s->block, s, b), (size_t)nq * k, ncclFloat32, s->comm, st));
-        COZO_NCCL(g_nccl.GroupEnd());
-      } else {
-        COZO_CUDA(cudaMemcpyAsync(set_ids(s->block, s, b), s->local_ids[b], (size_t)nq * k * 4, cudaMemcpyDeviceToDevice, st));
-        COZO_CUDA(cudaMemcpyAsync(set_dist(s->block, s, b), s->local_dist[b], (size_t)nq * k * 4, cudaMemcpyDeviceToDevice, st));
-      }
+      COZO_CUDA(cudaMemcpyAsync(set_ids(s->block, s, b), s->local_ids[b], (size_t)nq * k * 4, cudaMemcpyDeviceToDevice, st));
+      COZO_CUDA(cudaMemcpyAsync(set_dist<T>(s->block, s, b), local_dist, (size_t)nq * k * sizeof(T),
+                                cudaMemcpyDeviceToDevice, st));
     }
-    rc = cozo_gpu_topk_merge_dev(set_dist(s->block, s, b), set_ids(s->block, s, b), (uint32_t)s->world, nq, k,
-                                 s->d_offsets, d_out_ids + (size_t)q0 * k, d_out_dist + (size_t)q0 * k, st);
+    if constexpr (f64)
+      rc = topk_merge_f64_dev(set_dist<T>(s->block, s, b), set_ids(s->block, s, b), (uint32_t)s->world, nq, k,
+                              s->d_offsets, d_out_ids + (size_t)q0 * k, d_out_dist + (size_t)q0 * k, st);
+    else
+      rc = cozo_gpu_topk_merge_dev(set_dist<T>(s->block, s, b), set_ids(s->block, s, b), (uint32_t)s->world, nq, k,
+                                   s->d_offsets, d_out_ids + (size_t)q0 * k, d_out_dist + (size_t)q0 * k, st);
     if (rc) return rc;
   }
+  return 0;
+}
+
+// Argument checks every rank answers alike before any collective: the group's dtype was agreed at attach.
+static int check_group(cozo_gpu_shards* s, uint32_t k, uint32_t ef, int want_dtype) {
+  if (!s || !s->shard) return set_error(COZO_GPU_EINVAL, "no shard attached (cozo_gpu_hnsw_stage_sharded)");
+  if (s->dtype < 0) return set_error(COZO_GPU_EINVAL, "the shards of the group mix F32 and F64 indexes");
+  if (s->dtype != want_dtype)
+    return set_error(COZO_GPU_EINVAL, want_dtype ? "not an F64 group: use cozo_gpu_hnsw_search_sharded"
+                                                 : "F64 group: use cozo_gpu_hnsw_search_sharded_f64");
+  if (k == 0) return set_error(COZO_GPU_EINVAL, "k must be positive");
+  if (ef == 0) return set_error(COZO_GPU_EINVAL, "ef must be positive");
   return 0;
 }
 
@@ -368,7 +409,7 @@ extern "C" void cozo_gpu_shards_free(cozo_gpu_shards_t* s) {
   if (s->stream) cudaStreamSynchronize(s->stream);
   close_peers(s);
   void* ptrs[] = {s->block,    s->local_ids[0], s->local_ids[1], s->local_dist[0], s->local_dist[1], s->d_offsets,
-                  s->d_timeout, s->d_q,         s->d_out_ids,    s->d_out_dist,    s->d_qstats};
+                  s->d_timeout, s->d_q,         s->d_out_ids,    s->d_out_dist,    s->d_qstats,      s->d_mask};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   if (s->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(s->comm);
@@ -384,23 +425,26 @@ extern "C" int cozo_gpu_hnsw_stage_sharded(cozo_gpu_shards_t* s, cozo_gpu_hnsw_t
   int rc = ensure_init();
   if (rc) return rc;
   std::lock_guard<std::mutex> lk(s->mu);
-  uint64_t rows = local_shard->dev.n;
+  // every rank's (rows, dtype): [world][2] after the all-gather, this rank's pair at the end
+  const uint64_t mine[2] = {local_shard->dev.n, local_shard->f64 ? 1ull : 0ull};
   uint64_t* d_tmp = nullptr;
-  COZO_CUDA(cudaMalloc(&d_tmp, 8));
-  COZO_CUDA(cudaMemcpyAsync(d_tmp, &rows, 8, cudaMemcpyHostToDevice, s->stream));
+  COZO_CUDA(cudaMalloc(&d_tmp, 16 * ((size_t)s->world + 1)));
+  COZO_CUDA(cudaMemcpyAsync(d_tmp + 2 * s->world, mine, 16, cudaMemcpyHostToDevice, s->stream));
   if (s->world > 1)
-    COZO_NCCL(g_nccl.AllGather(d_tmp, s->d_offsets, 1, ncclUint64, s->comm, s->stream));
+    COZO_NCCL(g_nccl.AllGather(d_tmp + 2 * s->world, d_tmp, 2, ncclUint64, s->comm, s->stream));
   else
-    COZO_CUDA(cudaMemcpyAsync(s->d_offsets, d_tmp, 8, cudaMemcpyDeviceToDevice, s->stream));
-  std::vector<uint64_t> all(s->world);
-  COZO_CUDA(cudaMemcpyAsync(all.data(), s->d_offsets, (size_t)s->world * 8, cudaMemcpyDeviceToHost, s->stream));
+    COZO_CUDA(cudaMemcpyAsync(d_tmp, d_tmp + 2, 16, cudaMemcpyDeviceToDevice, s->stream));
+  std::vector<uint64_t> all(2 * (size_t)s->world);
+  COZO_CUDA(cudaMemcpyAsync(all.data(), d_tmp, (size_t)s->world * 16, cudaMemcpyDeviceToHost, s->stream));
   COZO_CUDA(cudaStreamSynchronize(s->stream));
   cudaFree(d_tmp);
   s->offsets.assign(s->world, 0);
   uint64_t acc = 0;
+  s->dtype = (int)all[1];
   for (int r = 0; r < s->world; ++r) {
     s->offsets[r] = acc;
-    acc += all[r];
+    acc += all[2 * r];
+    if ((int)all[2 * r + 1] != s->dtype) s->dtype = -1;
   }
   s->total_rows = acc;
   COZO_CUDA(cudaMemcpy(s->d_offsets, s->offsets.data(), (size_t)s->world * 8, cudaMemcpyHostToDevice));
@@ -419,14 +463,14 @@ extern "C" int cozo_gpu_shards_info(cozo_gpu_shards_t* s, int* rank, int* world,
   return 0;
 }
 
-extern "C" int cozo_gpu_hnsw_search_sharded_dev(cozo_gpu_shards_t* s, const float* queries_dev, uint32_t B, uint32_t k,
-                                                uint32_t ef, double radius, uint64_t* out_ids_dev, float* out_dist_dev,
-                                                uint32_t* per_query_stats_dev, void* stream) {
-  if (!s || !s->shard) return set_error(COZO_GPU_EINVAL, "no shard attached (cozo_gpu_hnsw_stage_sharded)");
-  if (k == 0) return set_error(COZO_GPU_EINVAL, "k must be positive");
-  if (ef == 0) return set_error(COZO_GPU_EINVAL, "ef must be positive");
+static int sharded_dev_entry(cozo_gpu_shards_t* s, const float* queries_dev, uint32_t B, uint32_t k, uint32_t ef,
+                             double radius, bool filtered, const uint32_t* row_mask_dev, uint64_t* out_ids_dev,
+                             float* out_dist_dev, uint32_t* per_query_stats_dev, void* stream) {
+  int rc = check_group(s, k, ef, 0);
+  if (rc) return rc;
+  if (filtered && s->shard->dev.n && !row_mask_dev) return set_error(COZO_GPU_EINVAL, "null row mask");
   if (B && (!queries_dev || !out_ids_dev || !out_dist_dev)) return set_error(COZO_GPU_EINVAL, "null buffer");
-  int rc = ensure_init();
+  rc = ensure_init();
   if (rc) return rc;
   if (B == 0) return 0;
   std::lock_guard<std::mutex> lk(s->mu);
@@ -435,7 +479,8 @@ extern "C" int cozo_gpu_hnsw_search_sharded_dev(cozo_gpu_shards_t* s, const floa
   COZO_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   COZO_CUDA(cudaEventRecord(e, (cudaStream_t)stream));
   COZO_CUDA(cudaStreamWaitEvent(s->stream, e, 0));
-  rc = sharded_search_dev(s, queries_dev, B, k, ef, radius, out_ids_dev, out_dist_dev, per_query_stats_dev);
+  rc = sharded_search_dev<float>(s, queries_dev, B, k, ef, radius, filtered ? row_mask_dev : nullptr, out_ids_dev,
+                                 out_dist_dev, per_query_stats_dev);
   if (!rc) {
     COZO_CUDA(cudaEventRecord(e, s->stream));
     COZO_CUDA(cudaStreamWaitEvent((cudaStream_t)stream, e, 0));
@@ -444,32 +489,36 @@ extern "C" int cozo_gpu_hnsw_search_sharded_dev(cozo_gpu_shards_t* s, const floa
   return rc;
 }
 
-extern "C" int cozo_gpu_hnsw_search_sharded(cozo_gpu_shards_t* s, const float* queries, uint32_t B, uint32_t k,
-                                            uint32_t ef, double radius, int root, uint64_t* out_ids, float* out_dist,
-                                            uint32_t* out_count, CozoGpuSearchStats* stats) {
-  if (!s || !s->shard) return set_error(COZO_GPU_EINVAL, "no shard attached (cozo_gpu_hnsw_stage_sharded)");
-  if (k == 0) return set_error(COZO_GPU_EINVAL, "k must be positive");
-  if (ef == 0) return set_error(COZO_GPU_EINVAL, "ef must be positive");
+// The host-pointer forms: T = float (F32 group) or double (F64 group); row_mask = this rank's filter verdicts, host
+// memory, nullptr = no filter.
+template <typename T>
+static int sharded_host_entry(cozo_gpu_shards_t* s, const T* queries, uint32_t B, uint32_t k, uint32_t ef,
+                              double radius, int root, bool filtered, const uint32_t* row_mask, uint64_t* out_ids,
+                              T* out_dist, uint32_t* out_count, CozoGpuSearchStats* stats) {
+  constexpr bool f64 = std::is_same<T, double>::value;
+  int rc = check_group(s, k, ef, f64 ? 1 : 0);
+  if (rc) return rc;
   if (root >= s->world) return set_error(COZO_GPU_EINVAL, "root %d out of range", root);
+  if (filtered && s->shard->dev.n && !row_mask) return set_error(COZO_GPU_EINVAL, "null row mask");
   const bool have_q = root < 0 || root == s->rank;
   if (B && have_q && !queries) return set_error(COZO_GPU_EINVAL, "null query buffer");
   if (B && ((out_ids == nullptr) != (out_dist == nullptr))) return set_error(COZO_GPU_EINVAL, "ids/dist must come together");
-  int rc = ensure_init();
+  rc = ensure_init();
   if (rc) return rc;
   if (stats) memset(stats, 0, sizeof(*stats));
   if (B == 0) return 0;
   std::lock_guard<std::mutex> lk(s->mu);
-  const uint32_t dim = s->shard->dev.dim;
-  const size_t qf = (size_t)B * dim;
-  if (s->q_floats < qf) {
+  cozo_gpu_hnsw* h = s->shard;
+  const size_t qf = (size_t)B * h->dev.dim;
+  if (s->q_bytes < qf * sizeof(T)) {
     if (s->d_q) cudaFree(s->d_q);
     s->d_q = nullptr;
-    s->q_floats = 0;
-    COZO_CUDA(cudaMalloc(&s->d_q, qf * 4));
-    s->q_floats = qf;
+    s->q_bytes = 0;
+    COZO_CUDA(cudaMalloc(&s->d_q, qf * sizeof(T)));
+    s->q_bytes = qf * sizeof(T);
   }
   if (s->out_rows < B || s->out_k < k) {
-    for (void* p : {(void*)s->d_out_ids, (void*)s->d_out_dist, (void*)s->d_qstats})
+    for (void* p : {(void*)s->d_out_ids, s->d_out_dist, (void*)s->d_qstats})
       if (p) cudaFree(p);
     s->d_out_ids = nullptr;
     s->d_out_dist = nullptr;
@@ -477,19 +526,51 @@ extern "C" int cozo_gpu_hnsw_search_sharded(cozo_gpu_shards_t* s, const float* q
     const size_t rows = std::max<size_t>(B, s->out_rows), kk = std::max<size_t>(k, s->out_k);
     s->out_rows = s->out_k = 0;
     COZO_CUDA(cudaMalloc(&s->d_out_ids, rows * kk * 8));
-    COZO_CUDA(cudaMalloc(&s->d_out_dist, rows * kk * 4));
+    COZO_CUDA(cudaMalloc(&s->d_out_dist, rows * kk * 8));
     COZO_CUDA(cudaMalloc(&s->d_qstats, rows * 16));
     s->out_rows = rows;
     s->out_k = kk;
   }
   cudaStream_t st = s->stream;
+  const uint32_t* d_mask = nullptr;
+  if (row_mask) {
+    const size_t words = ((size_t)h->dev.n + 31) / 32;
+    if (s->mask_words < words || !s->d_mask) {
+      if (s->d_mask) cudaFree(s->d_mask);
+      s->d_mask = nullptr;
+      s->mask_words = 0;
+      COZO_CUDA(cudaMalloc(&s->d_mask, std::max<size_t>(words, 1) * 4));
+      s->mask_words = words;
+    }
+    COZO_CUDA(cudaMemcpyAsync(s->d_mask, row_mask, words * 4, cudaMemcpyHostToDevice, st));
+    d_mask = s->d_mask;
+  }
+  // an F64 shard is searched with a workspace held for the whole call
+  struct Ws {
+    cozo_gpu_hnsw* h;
+    HnswWorkspace* ws;
+    cudaStream_t st;
+    ~Ws() {
+      if (ws) {
+        cudaStreamSynchronize(st);
+        hnsw_release_ws(h, ws);
+      }
+    }
+  } ws64{h, nullptr, st};
+  if (f64) {
+    ws64.ws = hnsw_acquire_ws(h);
+    if (!ws64.ws) return COZO_GPU_ECUDA;
+  }
   cudaEvent_t e0, e1;
   COZO_CUDA(cudaEventCreate(&e0));
   COZO_CUDA(cudaEventCreate(&e1));
-  if (have_q) COZO_CUDA(cudaMemcpyAsync(s->d_q, queries, qf * 4, cudaMemcpyHostToDevice, st));
-  if (root >= 0 && s->world > 1) COZO_NCCL(g_nccl.Broadcast(s->d_q, s->d_q, qf, ncclFloat32, root, s->comm, st));
+  T* d_q = static_cast<T*>(s->d_q);
+  T* d_out_dist = static_cast<T*>(s->d_out_dist);
+  if (have_q) COZO_CUDA(cudaMemcpyAsync(d_q, queries, qf * sizeof(T), cudaMemcpyHostToDevice, st));
+  if (root >= 0 && s->world > 1)
+    COZO_NCCL(g_nccl.Broadcast(d_q, d_q, qf, f64 ? ncclFloat64 : ncclFloat32, root, s->comm, st));
   COZO_CUDA(cudaEventRecord(e0, st));
-  rc = sharded_search_dev(s, s->d_q, B, k, ef, radius, s->d_out_ids, s->d_out_dist, s->d_qstats);
+  rc = sharded_search_dev<T>(s, d_q, B, k, ef, radius, d_mask, s->d_out_ids, d_out_dist, s->d_qstats, ws64.ws);
   if (rc) {
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
@@ -498,7 +579,7 @@ extern "C" int cozo_gpu_hnsw_search_sharded(cozo_gpu_shards_t* s, const float* q
   COZO_CUDA(cudaEventRecord(e1, st));
   if (out_ids) {
     COZO_CUDA(cudaMemcpyAsync(out_ids, s->d_out_ids, (size_t)B * k * 8, cudaMemcpyDeviceToHost, st));
-    COZO_CUDA(cudaMemcpyAsync(out_dist, s->d_out_dist, (size_t)B * k * 4, cudaMemcpyDeviceToHost, st));
+    COZO_CUDA(cudaMemcpyAsync(out_dist, d_out_dist, (size_t)B * k * sizeof(T), cudaMemcpyDeviceToHost, st));
   }
   std::vector<uint32_t> qs;
   if (stats) {
@@ -528,4 +609,43 @@ extern "C" int cozo_gpu_hnsw_search_sharded(cozo_gpu_shards_t* s, const float* q
     }
   }
   return 0;
+}
+
+extern "C" int cozo_gpu_hnsw_search_sharded_dev(cozo_gpu_shards_t* s, const float* queries_dev, uint32_t B, uint32_t k,
+                                                uint32_t ef, double radius, uint64_t* out_ids_dev, float* out_dist_dev,
+                                                uint32_t* per_query_stats_dev, void* stream) {
+  return sharded_dev_entry(s, queries_dev, B, k, ef, radius, false, nullptr, out_ids_dev, out_dist_dev,
+                           per_query_stats_dev, stream);
+}
+
+extern "C" int cozo_gpu_hnsw_search_sharded_filtered_dev(cozo_gpu_shards_t* s, const float* queries_dev, uint32_t B,
+                                                         uint32_t k, uint32_t ef, double radius,
+                                                         const uint32_t* row_mask_dev, uint64_t* out_ids_dev,
+                                                         float* out_dist_dev, uint32_t* per_query_stats_dev,
+                                                         void* stream) {
+  return sharded_dev_entry(s, queries_dev, B, k, ef, radius, true, row_mask_dev, out_ids_dev, out_dist_dev,
+                           per_query_stats_dev, stream);
+}
+
+extern "C" int cozo_gpu_hnsw_search_sharded(cozo_gpu_shards_t* s, const float* queries, uint32_t B, uint32_t k,
+                                            uint32_t ef, double radius, int root, uint64_t* out_ids, float* out_dist,
+                                            uint32_t* out_count, CozoGpuSearchStats* stats) {
+  return sharded_host_entry<float>(s, queries, B, k, ef, radius, root, false, nullptr, out_ids, out_dist, out_count,
+                                   stats);
+}
+
+extern "C" int cozo_gpu_hnsw_search_sharded_filtered(cozo_gpu_shards_t* s, const float* queries, uint32_t B,
+                                                     uint32_t k, uint32_t ef, double radius, int root,
+                                                     const uint32_t* row_mask, uint64_t* out_ids, float* out_dist,
+                                                     uint32_t* out_count, CozoGpuSearchStats* stats) {
+  return sharded_host_entry<float>(s, queries, B, k, ef, radius, root, true, row_mask, out_ids, out_dist, out_count,
+                                   stats);
+}
+
+extern "C" int cozo_gpu_hnsw_search_sharded_f64(cozo_gpu_shards_t* s, const double* queries, uint32_t B, uint32_t k,
+                                                uint32_t ef, double radius, int root, const uint32_t* row_mask,
+                                                uint64_t* out_ids, double* out_dist, uint32_t* out_count,
+                                                CozoGpuSearchStats* stats) {
+  return sharded_host_entry<double>(s, queries, B, k, ef, radius, root, false, row_mask, out_ids, out_dist, out_count,
+                                    stats);
 }

@@ -52,10 +52,11 @@ class ShardedTopK:
 
 def merge_lists(all_ids: np.ndarray, all_dist: np.ndarray, offsets, k: int):
     """[S,B,k] per-shard lists (local u32 ids, 0xFFFFFFFF padded, nearest first) -> global top-k:
-    ids u64 = offsets[s] + local id (UINT64_MAX padded), dist f32 (+inf padded); ties go to the lower shard."""
+    ids u64 = offsets[s] + local id (UINT64_MAX padded), dist f32, or f64 for f64 lists (+inf padded); ties go to the
+    lower shard."""
     S, B, _ = all_ids.shape
     out_i = np.full((B, k), np.uint64(0xFFFFFFFFFFFFFFFF), np.uint64)
-    out_d = np.full((B, k), np.inf, np.float32)
+    out_d = np.full((B, k), np.inf, np.float64 if np.asarray(all_dist).dtype == np.float64 else np.float32)
     for q in range(B):
         cand = [(float(all_dist[s, q, j]), s, j, int(offsets[s]) + int(all_ids[s, q, j]))
                 for s in range(S) for j in range(all_ids.shape[2]) if all_ids[s, q, j] != 0xFFFFFFFF]

@@ -269,7 +269,10 @@ int cozo_gpu_shards_info(cozo_gpu_shards_t* s, int* rank, int* world, int* excha
 
 /* Collective.  Attach this rank's shard — staged with cozo_gpu_hnsw_stage or built with
  * cozo_gpu_hnsw_build — to the communicator.  Shard r owns the global ids
- * [offset_r, offset_r + n_vectors_r) of the row-contiguous partition. */
+ * [offset_r, offset_r + n_vectors_r) of the row-contiguous partition.  Every rank also learns every
+ * shard's vec_dtype: the f32 searches below answer COZO_GPU_EINVAL on every rank of an F64 group,
+ * cozo_gpu_hnsw_search_sharded_f64 on every rank of an F32 group, and all of them on a group whose
+ * shards mix the two, before any collective. */
 int cozo_gpu_hnsw_stage_sharded(cozo_gpu_shards_t* s, cozo_gpu_hnsw_t* local_shard, uint64_t* out_global_offset,
                                 uint64_t* out_total_rows);
 
@@ -286,6 +289,32 @@ int cozo_gpu_hnsw_search_sharded(cozo_gpu_shards_t* s, const float* queries, uin
 int cozo_gpu_hnsw_search_sharded_dev(cozo_gpu_shards_t* s, const float* queries_dev, uint32_t B, uint32_t k,
                                      uint32_t ef, double radius, uint64_t* out_ids_dev, float* out_dist_dev,
                                      uint32_t* per_query_stats_dev, void* stream);
+
+/* Collective.  hnsw_knn with a `filter` over the whole sharded corpus: every shard runs the filtered
+ * search of cozo_gpu_hnsw_search_filtered (beam, radius, filter, then the first k) and the per-shard
+ * lists are merged as above, so k results per query and rank travel through the exchange.
+ * row_mask = this rank's verdicts over its LOCAL ids: bit (id & 31) of word id >> 5,
+ * [ceil(n_vectors_local/32)] words; NULL only on a rank whose shard is empty.  A NULL mask on a
+ * non-empty shard answers COZO_GPU_EINVAL on that rank alone: the caller makes the same call
+ * (filtered or not, same B, k, ef, radius, root) on every rank.  Other arguments as
+ * cozo_gpu_hnsw_search_sharded. */
+int cozo_gpu_hnsw_search_sharded_filtered(cozo_gpu_shards_t* s, const float* queries, uint32_t B, uint32_t k,
+                                          uint32_t ef, double radius, int root, const uint32_t* row_mask,
+                                          uint64_t* out_ids, float* out_dist, uint32_t* out_count,
+                                          CozoGpuSearchStats* stats);
+/* Same with the batch, the mask and the outputs in HBM; asynchronous, ordered after and before `stream`. */
+int cozo_gpu_hnsw_search_sharded_filtered_dev(cozo_gpu_shards_t* s, const float* queries_dev, uint32_t B, uint32_t k,
+                                              uint32_t ef, double radius, const uint32_t* row_mask_dev,
+                                              uint64_t* out_ids_dev, float* out_dist_dev,
+                                              uint32_t* per_query_stats_dev, void* stream);
+/* Collective.  hnsw_knn over a sharded corpus of F64 shards: every shard runs cozo_gpu_hnsw_search_f64
+ * (f64 queries, distances computed and returned in f64) and the lists are merged as above.  `queries`
+ * [B*dim] f64 is read on rank `root` and broadcast (root >= 0), or passed identically by every rank
+ * (root = -1).  row_mask nullable (no filter), otherwise as cozo_gpu_hnsw_search_sharded_filtered.
+ * out_ids [B*k] global ids padded with UINT64_MAX, out_dist [B*k] padded with +inf. */
+int cozo_gpu_hnsw_search_sharded_f64(cozo_gpu_shards_t* s, const double* queries, uint32_t B, uint32_t k, uint32_t ef,
+                                     double radius, int root, const uint32_t* row_mask, uint64_t* out_ids,
+                                     double* out_dist, uint32_t* out_count, CozoGpuSearchStats* stats);
 
 /* ---- graphs (FixedRule algorithms) -------------------------------------- */
 typedef struct cozo_gpu_graph cozo_gpu_graph_t;

@@ -107,6 +107,9 @@ extern "C" {
     pub fn cozo_gpu_hnsw_stage_sharded(s: *mut CozoGpuShards, local_shard: *mut CozoGpuHnsw, out_global_offset: *mut u64, out_total_rows: *mut u64) -> c_int;
     pub fn cozo_gpu_hnsw_search_sharded(s: *mut CozoGpuShards, queries: *const f32, B: u32, k: u32, ef: u32, radius: f64, root: c_int, out_ids: *mut u64, out_dist: *mut f32, out_count: *mut u32, stats: *mut CozoGpuSearchStats) -> c_int;
     pub fn cozo_gpu_hnsw_search_sharded_dev(s: *mut CozoGpuShards, queries_dev: *const f32, B: u32, k: u32, ef: u32, radius: f64, out_ids_dev: *mut u64, out_dist_dev: *mut f32, per_query_stats_dev: *mut u32, stream: *mut c_void) -> c_int;
+    pub fn cozo_gpu_hnsw_search_sharded_filtered(s: *mut CozoGpuShards, queries: *const f32, B: u32, k: u32, ef: u32, radius: f64, root: c_int, row_mask: *const u32, out_ids: *mut u64, out_dist: *mut f32, out_count: *mut u32, stats: *mut CozoGpuSearchStats) -> c_int;
+    pub fn cozo_gpu_hnsw_search_sharded_filtered_dev(s: *mut CozoGpuShards, queries_dev: *const f32, B: u32, k: u32, ef: u32, radius: f64, row_mask_dev: *const u32, out_ids_dev: *mut u64, out_dist_dev: *mut f32, per_query_stats_dev: *mut u32, stream: *mut c_void) -> c_int;
+    pub fn cozo_gpu_hnsw_search_sharded_f64(s: *mut CozoGpuShards, queries: *const f64, B: u32, k: u32, ef: u32, radius: f64, root: c_int, row_mask: *const u32, out_ids: *mut u64, out_dist: *mut f64, out_count: *mut u32, stats: *mut CozoGpuSearchStats) -> c_int;
     pub fn cozo_gpu_graph_stage(out: *mut *mut CozoGpuGraph, n: u32, m: u64, src: *const u32, dst: *const u32, w_or_null: *const f32) -> c_int;
     pub fn cozo_gpu_graph_free(g: *mut CozoGpuGraph);
     pub fn cozo_gpu_graph_stage_keys(out: *mut *mut CozoGpuGraph, m: u64, key_bytes: *const u8, key_off: *const u64, w_or_null: *const f32, undirected: i32, out_n: *mut u32) -> c_int;
