@@ -138,7 +138,7 @@ __global__ void __launch_bounds__(128, MINB) hnsw_search_kernel(HnswDev g, Searc
   }
   const int nvec4 = g.ld >> 2;
   // at run time: only if g.codes is set (then p.cns > 0); wide rows carry no codes
-  constexpr bool PRUNE = BULK && METRIC == COZO_GPU_L2 && NV > 0;
+  constexpr bool PRUNE = BULK && NV > 0;
 
   for (;;) {
     uint32_t qi = 0;
@@ -155,7 +155,13 @@ __global__ void __launch_bounds__(128, MINB) hnsw_search_kernel(HnswDev g, Searc
     QueryCodes qc;
     qc.a = reinterpret_cast<QueryPair*>(base + p.off_qcodes);
     if constexpr (PRUNE) {
-      if (g.codes) load_query_codes<NV>(q, g.ld, lane, qc);
+      if (g.codes) {
+        load_query_codes<NV>(q, g.ld, lane, qc);
+        if constexpr (METRIC != COZO_GPU_L2) {
+          if (lane == 0) *dot_query_of(qc) = code_dot_query<METRIC>(qc.c, qnorm);
+          __syncwarp();
+        }
+      }
     }
     w.len = 0;
     w.cursor = 0;
@@ -449,15 +455,17 @@ static void codes_drop(cozo_gpu_hnsw* h) {
   h->dev.codes = nullptr;
 }
 
-// Room for `rows` code rows, keeping rows [0, n).  Only L2 f32 indexes with CODES_MIN_LD <= ld <= 2048 carry codes.  A failed
-// allocation leaves
-// the index without codes: it is then searched without pruning, with the same results.
-void hnsw_codes_reserve(cozo_gpu_hnsw* h, uint32_t rows) {
+// Only f32 indexes (of any metric) with CODES_MIN_LD <= ld <= 2048 carry codes: the pruning bound (hnsw_codes.cuh) is
+// argued for ld <= REG_QUERY_MAX_LD, and the wide kernels do not prune.  A failed allocation leaves the index without
+// codes: it is then searched without pruning, with the same results.
+static bool codes_eligible(const cozo_gpu_hnsw* h) {
+  const HnswDev& g = h->dev;
+  return !h->f64 && g.ld >= CODES_MIN_LD && g.ld <= REG_QUERY_MAX_LD && !h->codes_failed;
+}
+
+// Room for `rows` code rows, keeping rows [0, n).
+static void codes_grow(cozo_gpu_hnsw* h, uint32_t rows) {
   HnswDev& g = h->dev;
-  // the pruning bound (hnsw_codes.cuh) is argued for ld <= REG_QUERY_MAX_LD, and the wide kernels do not prune
-  if (h->f64 || g.metric != COZO_GPU_L2 || g.ld < CODES_MIN_LD || g.ld > REG_QUERY_MAX_LD || h->codes_failed ||
-      rows <= h->codes_rows)
-    return;
   uint8_t* nc = nullptr;
   if (cudaMalloc(&nc, (size_t)rows * g.code_ld) != cudaSuccess) {
     cudaGetLastError();  // not sticky: clear it
@@ -476,12 +484,36 @@ void hnsw_codes_reserve(cozo_gpu_hnsw* h, uint32_t rows) {
   g.codes = nc;
 }
 
+// Room for `rows` code rows wherever the vector rows grow.  An L2 index gets its codes here when it is staged; a Cosine
+// or IP index gets them from its first search (hnsw_codes_ensure), so that staging and building it take the memory they
+// took before those metrics pruned, and until then it has none to grow.
+void hnsw_codes_reserve(cozo_gpu_hnsw* h, uint32_t rows) {
+  if (!codes_eligible(h) || rows <= h->codes_rows || (h->dev.metric != COZO_GPU_L2 && !h->d_codes)) return;
+  codes_grow(h, rows);
+}
+
+// A Cosine or IP index without code rows: make them for every allocated row and quantise the live ones, once, and wait
+// for that on the default stream (the search may run on any stream).  Searches of the index all pass here first, so the
+// mutex also orders the pointer's publication before their reads of h->dev.
+void hnsw_codes_ensure(cozo_gpu_hnsw* h) {
+  if (h->dev.metric == COZO_GPU_L2) return;
+  std::lock_guard<std::mutex> lk(h->codes_mu);
+  const uint32_t rows = std::max(h->cap_n, h->dev.n);
+  if (h->d_codes || !codes_eligible(h) || rows == 0) return;
+  codes_grow(h, rows);
+  hnsw_codes_fill(h, 0, h->dev.n);
+  if (h->d_codes && cudaStreamSynchronize(0) != cudaSuccess) {
+    cudaGetLastError();
+    codes_drop(h);
+  }
+}
+
 // Re-quantise the code rows of the vector rows just written (ids = nullptr: rows first .. first+count-1), on the
 // default stream, after the writes to d_vec.
 void hnsw_codes_fill(cozo_gpu_hnsw* h, uint32_t first, uint32_t count, const uint32_t* d_ids) {
   const HnswDev& g = h->dev;
   if (!g.codes || !count) return;
-  quantize_rows_kernel<<<(count + 127) / 128, 128>>>(h->d_vec, g.ld, h->d_codes, d_ids, first, count);
+  quantize_rows_kernel<<<(count + 127) / 128, 128>>>(h->d_vec, g.ld, h->d_codes, d_ids, first, count, g.metric);
   if (cudaGetLastError() != cudaSuccess) codes_drop(h);
 }
 
@@ -489,8 +521,9 @@ int hnsw_launch_search(cozo_gpu_hnsw* h, HnswWorkspace* ws, const float* d_q, ui
                        double radius, uint32_t* d_ids, float* d_dist, uint32_t* d_count, uint32_t* d_qstats,
                        cudaStream_t stream, const ScatterDest* scatter, const uint32_t* d_filter_mask) {
   const DeviceInfo& di = device_info();
-  const HnswDev& g = h->dev;
   if (B == 0) return 0;
+  hnsw_codes_ensure(h);
+  const HnswDev& g = h->dev;
   // mode 0: plain ld.global rows, 1: warp per query + TMA ring, 2: CTA per query (cooperative),
   // -1 (default): cooperative when the batch cannot give every resident warp slot a query
   int64_t mode = get_option("hnsw.mode", -1);
@@ -573,11 +606,12 @@ int hnsw_launch_search(cozo_gpu_hnsw* h, HnswWorkspace* ws, const float* d_q, ui
       // The fixed-point query (QueryCodes, 256 B per 128 elements) is taken from the code ring: at config 2 (D = 768,
       // ef 200) that leaves 2 f32 + 5 code stages (7 before); hnsw.stages=1 (1 + 2) measured 0.9 % slower
       // (tools/sweep.py).
-      // [fd][fi][pend][bars ns][code bars <= 16][fixed-point query][f32 ring ns][code ring cns]
+      // [fd][fi][pend][bars ns][code bars <= 16][CodeDotQuery: Cosine and IP][fixed-point query][f32 ring ns]
+      // [code ring cns]
       const uint32_t budget = p.warp_smem;
       ns = std::min<uint32_t>(ns, 2);
       p.off_cbars = p.off_bars + ns * 8;
-      p.off_qcodes = p.off_cbars + 16 * 8;
+      p.off_qcodes = p.off_cbars + 16 * 8 + (g.metric == COZO_GPU_L2 ? 0 : (uint32_t)sizeof(CodeDotQuery));
       p.off_ring = round_up(p.off_qcodes + (g.ld / 4 + 31) / 32 * 256, 128);
       p.off_cring = p.off_ring + ns * g.ld * 4;  // a multiple of 16: ld is a multiple of 4
       const uint32_t room = budget > p.off_cring ? budget - p.off_cring : 0;

@@ -1,14 +1,16 @@
-// hnsw_codes.cuh — the compact uint8 copy of an index's f32 vectors and the exact lower bound on the L2 distance that
-// lets the search reject a neighbour without fetching its f32 row.
+// hnsw_codes.cuh — the compact uint8 copy of an index's f32 vectors and the exact bounds on the search kernel's distance
+// (L2, Cosine and IP) that let the search reject a neighbour without fetching its f32 row.
 //
 // Layout: one code row per vector, code_row_bytes(ld) = 16 + round_up(ld, 16) bytes, so that a row is one
 // cp.async.bulk (16-byte aligned, a multiple of 16 bytes long):
-//   float lo, scale, err, X2     the row header
+//   float lo, scale, err, X      the row header; X is X2 on an L2 index and Xn on a Cosine or IP index
 //   uint8 c[ld]                  one code per element of the f32 row, padding elements included; zero padded
 // Element j dequantises to  x~_j = fmaf((float)c_j, scale, lo)  (code_value), and in exact arithmetic to
 // x^_j = lo + scale c_j.  err >= ||x - x~||_2 and err >= ||x - x^||_2 over all ld elements, computed in f64 and rounded
-// up; X2 <= ||x^||^2, computed in f64 and rounded down.  A row holding NaN or +-inf (or whose range or X2 overflows f32)
-// gets err = +inf and is never pruned.
+// up.  L2: X2 <= ||x^||^2, computed in f64 and rounded down.  Cosine and IP: Xn >= ||x||_2, computed in f64 and rounded
+// up, so that ||x|| lies in [Xn (1 - 2^-22), Xn].  A row holding NaN or +-inf (or whose range or X2 overflows f32) gets
+// err = +inf and is never pruned; so does a Cosine or IP row with Xn outside [CODE_XN_MIN, CODE_XN_MAX] (a zero row
+// among them).
 #pragma once
 #include <math.h>
 
@@ -31,8 +33,13 @@ __host__ __device__ inline float code_value(uint32_t c, float lo, float scale) {
 
 __host__ __device__ inline bool code_finite(float v) { return fabsf(v) <= 3.40282347e38f; }
 
-// Affine per-row quantisation of x[0..ld) into `out` (code_row_bytes(ld) bytes).
-__host__ __device__ inline void quantize_row(const float* x, uint32_t ld, uint8_t* out) {
+// The range of Xn inside which a Cosine or IP row can be pruned (code_dot_prunes): below it the kernel's f32 sum of
+// squares could lose more than REL to underflow, above it the f32 dot product with a query of norm <= CODE_XN_MAX could
+// overflow (both norms <= 2^63 keep every partial sum below 2^127).
+constexpr double CODE_XN_MIN = 0x1p-40, CODE_XN_MAX = 0x1p63;
+
+// Affine per-row quantisation of x[0..ld) into `out` (code_row_bytes(ld) bytes), with the header word 3 of `metric`.
+__host__ __device__ inline void quantize_row(const float* x, uint32_t ld, uint8_t* out, int metric = COZO_GPU_L2) {
   bool finite = true;
   float lo = x[0], hi = x[0];
   for (uint32_t j = 0; j < ld; ++j) {
@@ -45,7 +52,7 @@ __host__ __device__ inline void quantize_row(const float* x, uint32_t ld, uint8_
   if (!code_finite(scale)) finite = false;
   if (!finite) lo = scale = 0.f;
   uint8_t* c = out + CODE_HDR;
-  double ss = 0.0, x2 = 0.0;
+  double ss = 0.0, x2 = 0.0, n2 = 0.0;
   for (uint32_t j = 0; j < ld; ++j) {
     uint32_t cj = 0;
     if (scale > 0.f) {
@@ -60,6 +67,7 @@ __host__ __device__ inline void quantize_row(const float* x, uint32_t ld, uint8_
     ss += e * e;
     const double xe = fma((double)scale, (double)cj, (double)lo);
     x2 += xe * xe;
+    n2 += (double)x[j] * (double)x[j];  // exact products
   }
   for (uint32_t j = ld; j < code_row_bytes(ld) - CODE_HDR; ++j) c[j] = 0;
   // ss and x2 are sums of non-negative terms and carry at most (2 ld + 6) f64 roundings, far below the 2^-30 the
@@ -75,6 +83,15 @@ __host__ __device__ inline void quantize_row(const float* x, uint32_t ld, uint8_
     if (!code_finite(X2)) {
       err = INFINITY;
       X2 = 0.f;
+    }
+    if (metric != COZO_GPU_L2) {  // X2 is replaced by Xn
+      const double xn = sqrt(n2 * (1.0 + 0x1p-30)) * (1.0 + 0x1p-30);
+      X2 = (float)xn;
+      if ((double)X2 < xn) X2 = nextafterf(X2, INFINITY);
+      if (!((double)X2 >= CODE_XN_MIN && (double)X2 <= CODE_XN_MAX)) {
+        err = INFINITY;
+        X2 = 0.f;
+      }
     }
   }
   float* hdr = reinterpret_cast<float*>(out);
@@ -205,14 +222,82 @@ __host__ __device__ inline bool code_int_prunes(const CodeQuery& cq, int32_t S, 
   return dlo <= 1.7976931348623157e308 && dlo >= r * r;
 }
 
+// ---- the bound for Cosine and IP: an upper bound on the kernel's f32 dot product ---------------------------------------
+// What the kernel computes (finish<METRIC>, hnsw_device.cuh): a = the f32 dot product q.x (lane-strided fmaf chains over
+// all ld elements, then the shuffle tree), b = the f32 sum of x_j^2 in the same order, qnorm = load_query's f32 sum of
+// q_j^2, and then  IP: d = (float)(1 - (double)a),  Cosine: d = (float)(1 - (double)a / sqrt((double)qnorm (double)b)).
+// Both are non-increasing in a.  The test proves d >= worst from an upper bound U >= a:
+//   Exact arithmetic: q.x = q^.x^ + (q - q^).x + q^.(x - x^), with q^.x^ = s_q (lo sum_j a_j + scale S) (CodeQuery) exact,
+//   |(q - q^).x| <= e_q ||x|| <= e_q Xn  and  |q^.(x - x^)| <= ||q^|| err,  ||q^|| = sqrt(Q2) (Q2 exact in f64).
+//   Rounding of a: a sum of ld/32 + 5 roundings per term, so |a - q.x| <= (ld/32 + 7) 2^-24 sum_j |q_j x_j| <=
+//   REL ||q|| ||x|| <= REL (||q^|| + e_q) Xn for ld <= 2048 (the L2 argument), plus 1e-36 for subnormal underflow.  The
+//   norms are at most CODE_XN_MAX = 2^63 (the row's by quantize_row, the query's by code_dot_query), so no partial sum
+//   overflows.  So
+//     U = s_q (lo sum a + scale S) + Xn (e_q + REL (||q^|| + e_q)) + ||q^|| err + 1e-36 >= a.
+//   The f64 evaluation of U takes under 16 roundings, each at most 2^-53 of M = |lo s_q sum a| + |s_q scale S| +
+//   Xn (e_q + ...) + ||q^|| err + 1e-36; adding 2^-45 M covers them.
+// IP: a <= U <= T = 1 - worst exactly  =>  1 - (double)a >= worst (rounding is monotone and worst is a float)  =>
+//   d >= worst.  T is taken as the f64 1 - worst lowered by 2^-50 of itself (the subtraction rounds at 2^-53).
+// Cosine: with the kernel's qnorm known, s = sqrt(qnorm b) rounds once (qnorm b is exact in f64), and so does a / s.
+//   b is within REL of ||x||^2 (a sum of non-negative terms; Xn >= CODE_XN_MIN keeps underflow below 2^-61 of it), and
+//   ||x|| is in [Xn (1 - 2^-22), Xn], so  sqrt(qnorm) Xn (1 - 2^-13) <= s (1 -+ 2^-53) <= sqrt(qnorm) Xn (1 + 2^-13)
+//   with room to spare.  If U >= 0: a / s <= U / s_min, and the rounded quotient is at most (1 + 2^-53) of that, so
+//   U <= T sqrt(qnorm) Xn (1 - 2^-13) suffices.  If U < 0: a / s <= U / s_max and the rounded quotient is at most
+//   (1 - 2^-53) of that, so U <= T sqrt(qnorm) Xn (1 + 2^-13) suffices.  Then (double)a / s <= T, and as for IP
+//   d >= worst.  The f64 steps from worst to T sqrt(qnorm) Xn (1 -+ 2^-13) round 6 times, far inside the margin that
+//   2^-13 leaves over REL + 2^-22.
+//   |a / s| lies in [2^-275, 2^277] unless a = 0, so the quotient neither underflows nor overflows.
+// Nothing prunes when: err = +inf (non-finite rows, rows outside the Xn range, zero rows), e_q = +inf (non-finite
+// queries), the query's norm bound exceeds CODE_XN_MAX, Cosine with qnorm = 0 (or NaN), worst NaN or +-inf, or U NaN.
+// Tightness: the Cauchy-Schwarz term ||q^|| err is larger than the L2 bound's error term on most data.
+constexpr double CODE_COS_LO = 1.0 - 0x1p-13, CODE_COS_HI = 1.0 + 0x1p-13;
+
+struct CodeDotQuery {
+  double sq;   // s_q
+  double ssa;  // s_q sum a_j (exact: s_q is a power of two)
+  double qn;   // ||q^|| = sqrt(Q2)
+  double k1;  // e_q + REL (||q^|| + e_q): the factor of Xn in U
+  double rq;  // IP: 1; Cosine: sqrt(qnorm); NaN: nothing is pruned for this query
+};
+
+// the per-query constants of code_dot_prunes, from the fixed-point query and the kernel's f32 qnorm
+template <int METRIC>
+__host__ __device__ inline CodeDotQuery code_dot_query(const CodeQuery& cq, float qnorm) {
+  CodeDotQuery d;
+  d.sq = 0.5 * cq.sq2;
+  d.ssa = d.sq * (double)cq.suma;
+  d.qn = sqrt(cq.q2);
+  d.k1 = cq.eq + CODE_REL * (d.qn + cq.eq);
+  const bool ok = d.qn + cq.eq <= CODE_XN_MAX && (METRIC == COZO_GPU_IP || qnorm > 0.f);
+  d.rq = !ok ? (double)NAN : METRIC == COZO_GPU_IP ? 1.0 : sqrt((double)qnorm);
+  return d;
+}
+
+// what U is compared with, once per value of the beam's worst distance: T = 1 - worst (lowered), times rq
+__host__ __device__ inline double code_dot_radius(const CodeDotQuery& cd, float worst) {
+  if (!code_finite(worst)) return NAN;
+  const double t = 1.0 - (double)worst;
+  return (t - fabs(t) * 0x1p-50) * cd.rq;
+}
+
+// Whether the row with header hdr = {lo, scale, err, Xn} and S = sum a_j c_j can be dropped; R = code_dot_radius.
+template <int METRIC>
+__host__ __device__ inline bool code_dot_prunes(const CodeDotQuery& cd, int32_t S, const float* hdr, double R) {
+  const double x = (double)hdr[0] * cd.ssa, y = cd.sq * ((double)hdr[1] * (double)S), xn = (double)hdr[3];
+  const double e = xn * cd.k1 + cd.qn * (double)hdr[2] + 1e-36;
+  const double u = (x + y) + e + 0x1p-45 * (fabs(x) + fabs(y) + e);
+  if (METRIC == COZO_GPU_IP) return u <= R;
+  return u <= R * xn * (u >= 0.0 ? CODE_COS_LO : CODE_COS_HI);
+}
+
 // Fills the code rows of vectors ids[i] (ids == nullptr: first + i) for i < count.  One thread per row: this runs
 // once per write of the vectors, not per search.
 static __global__ void quantize_rows_kernel(const float* vec, uint32_t ld, uint8_t* codes, const uint32_t* ids,
-                                            uint32_t first, uint32_t count) {
+                                            uint32_t first, uint32_t count, int metric) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
   const size_t r = ids ? ids[i] : first + i;
-  quantize_row(vec + r * ld, ld, codes + r * code_row_bytes(ld));
+  quantize_row(vec + r * ld, ld, codes + r * code_row_bytes(ld), metric);
 }
 
 }  // namespace cozo

@@ -370,6 +370,11 @@ struct QueryCodes {
   QueryPair* a;
   CodeQuery c;
 };
+// Cosine and IP: the query's CodeDotQuery (code_dot_query) sits in shared memory right before a[], read where it is used
+// (in registers the pruned kernel spills)
+__device__ __forceinline__ CodeDotQuery* dot_query_of(const QueryCodes& qc) {
+  return reinterpret_cast<CodeDotQuery*>(qc.a) - 1;
+}
 
 // code_query_prepare of hnsw_codes.cuh, across the warp: the same per-element functions, the sums in lane order
 template <int NV>
@@ -473,13 +478,14 @@ __device__ __forceinline__ void code_idot2(const QueryCodes& qc, const uint8_t* 
 #endif
 }
 
-// One 32-id adjacency chunk of a pruned hop (L2, codes present, beam full), as one stream per warp.  `id` is this lane's
+// One 32-id adjacency chunk of a pruned hop (codes present, beam full), as one stream per warp.  `id` is this lane's
 // neighbour id (NONE = idle), `validmask` the lanes that hold one.
 //   * The code rows of the first w.cns valid ids are issued before the visited test, so their fetch overlaps the
 //     atomicOr round trip.  Those that turn out to be visited are waited for and discarded (not scored, not counted);
 //     later ids are fetched only if they are unvisited.  Stream position p holds w.pend[p], bit 31 set = discard.
-//   * Each code row is bounded from below (hnsw_codes.cuh, code_int_prunes: from the exact integer product of the code
-//     row with the fixed-point query qc) against the beam's worst distance AT THAT MOMENT.  With a
+//   * Each code row's distance is bounded from below (hnsw_codes.cuh, code_int_prunes for L2, code_dot_prunes for Cosine
+//     and IP: from the exact integer product of the code row with the fixed-point query qc) against the beam's worst
+//     distance AT THAT MOMENT.  With a
 //     full beam fd[len-1] only decreases, and a neighbour's admission test `d < fd[len-1]` comes after every earlier
 //     survivor's admission, so the value tested here is at least the one its admission would face: a dropped
 //     neighbour could not have been admitted.
@@ -487,9 +493,9 @@ __device__ __forceinline__ void code_idot2(const QueryCodes& qc, const uint8_t* 
 //     as soon as it has landed (polled, never waited for while code rows remain); the rest are drained at the end.
 //     Admissions therefore happen in neighbour order with the live bound, exactly as without pruning: ids, distances
 //     and the traversal counters are unchanged; only the number of f32 rows fetched can go down.
-template <int NV>
-__device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const float4 (&q)[NV], const QueryCodes& qc,
-                                            uint32_t ef, uint32_t id, uint32_t validmask, int lane) {
+template <int NV, int METRIC>
+__device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const float4 (&q)[NV], float qnorm,
+                                            const QueryCodes& qc, uint32_t ef, uint32_t id, uint32_t validmask, int lane) {
   const int nvec4 = g.ld >> 2;
   const uint32_t crow = g.code_ld, row_bytes = g.ld * 4;
   const uint32_t lt = (1u << lane) - 1;
@@ -515,7 +521,16 @@ __device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const 
   HOP_ADD(w, HC_VISIT, t0);
 
   uint32_t fq = 0, fin = 0;  // bits by stream position: survivors whose f32 row is queued / in flight (in order)
-  double WE = code_int_radius(qc.c, w.fd[ef - 1]);
+  // the per-row test and what it compares with, recomputed whenever the beam's worst distance changes
+  auto radius = [&](float worst) {
+    if constexpr (METRIC == COZO_GPU_L2) return code_int_radius(qc.c, worst);
+    else return code_dot_radius(*dot_query_of(qc), worst);
+  };
+  auto prunes = [&](int32_t S, const float* hdr, double WE) {
+    if constexpr (METRIC == COZO_GPU_L2) return code_int_prunes(qc.c, S, hdr, WE);
+    else return code_dot_prunes<METRIC>(*dot_query_of(qc), S, hdr, WE);
+  };
+  double WE = radius(w.fd[ef - 1]);
   // f32 ring: slot w.head holds the oldest row in flight, popc(fin) rows are in flight
   auto f32_issue = [&]() {
     while (fq && __popc(fin) < w.ns) {
@@ -539,14 +554,18 @@ __device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const 
     HOP_T(t2);
     const float4* row = reinterpret_cast<const float4*>(w.ring + (size_t)w.head * g.ld);
     // above NV = 6 the loads-first form needs more registers than the kernel has (it spills)
-    const float d = NV > 6 ? dist_smem<NV, COZO_GPU_L2>(q, row, lane, nvec4, 0.f) : dist_smem_l2<NV>(q, row, lane, nvec4);
+    float d;
+    if constexpr (METRIC == COZO_GPU_L2)
+      d = NV > 6 ? dist_smem<NV, COZO_GPU_L2>(q, row, lane, nvec4, 0.f) : dist_smem_l2<NV>(q, row, lane, nvec4);
+    else
+      d = dist_smem<NV, METRIC>(q, row, lane, nvec4, qnorm);
     if (++w.head == w.ns) w.head = 0;
     const uint32_t nid = w.pend[__ffs(fin) - 1];
     fin &= fin - 1;
     __syncwarp();
     if (d < w.fd[ef - 1]) {  // hnsw.rs:575-581 (the beam stays full)
       sorted_insert(w, ef, d, nid, lane);
-      WE = code_int_radius(qc.c, w.fd[ef - 1]);
+      WE = radius(w.fd[ef - 1]);
     }
     HOP_ADD(w, HC_FSCORE, t2);
   };
@@ -585,11 +604,11 @@ __device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const 
     const uint32_t p0 = w.pend[c], p1 = two ? w.pend[c + 1] : EXPANDED;
     __syncwarp();  // every lane is done with the two slots before lane 0 refills them
     if (!(p0 & EXPANDED)) {
-      if (code_int_prunes(qc.c, S0, &h0.x, WE)) w.pruned++;
+      if (prunes(S0, &h0.x, WE)) w.pruned++;
       else fq |= 1u << c;
     }
     if (!(p1 & EXPANDED)) {
-      if (code_int_prunes(qc.c, S1, &h1.x, WE)) w.pruned++;
+      if (prunes(S1, &h1.x, WE)) w.pruned++;
       else fq |= 1u << (c + 1);
     }
     const uint32_t step = two ? 2 : 1;
@@ -612,7 +631,7 @@ __device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const 
 
 // hnsw_search_level (hnsw.rs:539-587) for one query held in registers.
 // `level` 0 is the bottom layer.  On entry the sorted array holds found_nn.
-// PRUNE (L2 with the bulk ring): when g.codes is set, the chunks of a hop that find the beam full run prune_chunk, which
+// PRUNE (the bulk ring, register query): when g.codes is set, the chunks of a hop that find the beam full run prune_chunk, which
 // fetches f32 rows only for the neighbours whose code row cannot rule out admission.
 // qc: the query's fixed-point form (load_query_codes), read only by prune_chunk.
 // NV = 0: the query is a WideQuery (no pruning).
@@ -679,7 +698,7 @@ __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const
       w.nbr_reads += __popc(validmask);
       if constexpr (PRUNE) {
         if (g.codes && w.len == ef) {
-          prune_chunk<NV>(g, w, q, *qc, ef, id, validmask, lane);
+          prune_chunk<NV, METRIC>(g, w, q, qnorm, *qc, ef, id, validmask, lane);
           __syncwarp();
           continue;
         }

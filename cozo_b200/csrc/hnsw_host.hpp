@@ -35,11 +35,14 @@ struct cozo_gpu_hnsw {
   // owned device buffers
   float* d_vec = nullptr;
   bool vec_owned = true;
-  // uint8 code rows of an L2 f32 index (hnsw_codes.cuh), one per row of d_vec, written wherever d_vec is;
-  // dev.codes = nullptr when there are none (other metrics, F64, or an allocation that failed)
+  // uint8 code rows of an f32 index (hnsw_codes.cuh, header in the index's metric), one per row of d_vec, written
+  // wherever d_vec is; made at staging for L2, by the first search for Cosine and IP (hnsw_codes_ensure, under
+  // codes_mu); dev.codes = nullptr when there are none (not yet searched, rows narrower than CODES_MIN_LD or wider
+  // than 2048, F64, or an allocation that failed)
   uint8_t* d_codes = nullptr;
   uint32_t codes_rows = 0;     // allocated rows
   bool codes_failed = false;   // an allocation or a fill failed: the index stays without codes
+  std::mutex codes_mu;
   // F64 vector index (VecElementType::F64): payloads as doubles, searched by hnsw_f64.cu only
   double* d_vec64 = nullptr;
   uint32_t ld64 = 0;
@@ -138,5 +141,6 @@ void hnsw_release_ws(cozo_gpu_hnsw* h, HnswWorkspace* ws);
 int hnsw_ws_reserve(HnswWorkspace* ws, size_t vis_words, size_t vlog_words, cudaStream_t stream);
 int hnsw_ensure_build_state(cozo_gpu_hnsw* h);
 void hnsw_codes_reserve(cozo_gpu_hnsw* h, uint32_t rows);
+void hnsw_codes_ensure(cozo_gpu_hnsw* h);
 void hnsw_codes_fill(cozo_gpu_hnsw* h, uint32_t first, uint32_t count, const uint32_t* d_ids = nullptr);
 }  // namespace cozo

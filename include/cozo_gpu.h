@@ -127,7 +127,7 @@ int cozo_gpu_hnsw_search(cozo_gpu_hnsw_t* h, const float* queries, uint32_t B, u
 /* Same with every buffer already resident in HBM; asynchronous on `stream`
  * (a cudaStream_t, NULL = legacy default stream).  per_query_stats_dev: nullable
  * u32 [B*4] = {dist_evals, nodes_expanded, nbr_reads, f32 rows fetched}; the last is below dist_evals when
- * the L2 search rejected neighbours from their uint8 code rows alone, and equals it otherwise. */
+ * the search (of any metric) rejected neighbours from their uint8 code rows alone, and equals it otherwise. */
 int cozo_gpu_hnsw_search_dev(cozo_gpu_hnsw_t* h, const float* queries_dev, uint32_t B, uint32_t k, uint32_t ef,
                              double radius, uint32_t* out_ids_dev, float* out_dist_dev, uint32_t* out_count_dev,
                              uint32_t* per_query_stats_dev, void* stream);

@@ -64,6 +64,17 @@ for nh, gs, win in ((64, 256, 512), (0, 64, 64), (1024, 4096, 3001)):
     capi.set_option("pagerank.chunk", 1024)
     hub.pagerank(0.85, 0.0, 2)
     gg.pagerank(0.85, 1e-4, 3)
+# the pruned search (code rows: 512 <= ld <= 2048) on an index of each metric, also after writes of the vectors
+for metric in (capi.L2, capi.COSINE, capi.IP):
+    X = rng.random((1200, 516), dtype=np.float32) - (0.0 if metric == capi.L2 else 0.3)
+    g = capi.HnswIndex.build(X, metric=metric, m=8, ef_construction=40)
+    Q = rng.random((40, 516), dtype=np.float32) - (0.0 if metric == capi.L2 else 0.3)
+    capi.set_option("hnsw.mode", 1)
+    g.search(Q, 5, 16)
+    g.update(np.array([2, 700], np.uint32), rng.random((2, 516), dtype=np.float32))
+    g.insert_at(np.array([10], np.uint32), rng.random((1, 516), dtype=np.float32))
+    g.search(Q, 5, 16, row_pass=rng.random(1201) < 0.5)
+    capi.set_option("hnsw.mode", -1)
 # filter mask in every search mode, F64 index, the compacted-frontier SSSP, sharded operator at world size 1
 X = rng.random((1500, 48), dtype=np.float32)
 g = capi.HnswIndex.build(X, m=8, ef_construction=40)
