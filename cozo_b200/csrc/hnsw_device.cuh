@@ -12,7 +12,8 @@
 //     (hnsw.rs:575-581) is applied in neighbour order with the live bound, so the
 //     traversal, dist_evals and nodes_expanded equal the reference's.
 //   * `visited` (hnsw.rs:549) is a per-warp bitmap in HBM, set with atomicOr and
-//     cleared at the end of every layer through a log of the ids that were set.
+//     cleared at the end of every layer (visit_clear), through a log of the ids
+//     that were set or by sweeping the whole bitmap.
 #pragma once
 #include "common.cuh"
 #include "hnsw_codes.cuh"
@@ -345,9 +346,15 @@ __device__ __forceinline__ bool visit_mark(WarpCtx& w, uint32_t id, int lane, ui
   return isnew;
 }
 
+// Clearing by the log costs one random atomic per logged id; by the sweep, one coalesced 16-byte store per 4 words.  A
+// random atomic on a bitmap that has left L2 costs about as much as half a 784-byte row gather (tools/gather_ceiling.py
+// --visited), far more than the 128 bytes of sweep that replace it, so the log is used only for layers that set fewer
+// than one id per VISIT_SWEEP_WORDS words (the upper layers; at 1 M rows, fewer than ~980 ids).
+constexpr uint32_t VISIT_SWEEP_WORDS = 32;
+
 __device__ __forceinline__ void visit_clear(WarpCtx& w, int lane) {
   __syncwarp();
-  if (w.nlog <= w.logcap && w.nlog * 4 <= w.nwords) {
+  if (w.nlog <= w.logcap && w.nlog * VISIT_SWEEP_WORDS <= w.nwords) {
     for (uint32_t i = lane; i < w.nlog; i += 32) atomicAnd(&w.vis[w.vlog[i] >> 5], 0u);
   } else {
     uint4 z = make_uint4(0, 0, 0, 0);
