@@ -7,7 +7,7 @@
 // contributions, out-degrees and the rows of the in-CSR are slot-indexed; scores are un-permuted once
 // at the end.  Two iteration engines over it:
 //
-//   mode 1 (default)  PROPAGATION BLOCKING with TMA-staged contribution tiles.  The random 4-byte gather
+//   mode 1            PROPAGATION BLOCKING with TMA-staged contribution tiles.  The random 4-byte gather
 //     of the pull (one 32-byte L2 sector per in-edge) is replaced by streaming passes:
 //       sources by slot:  H = the first NH slots (hub sources, ~30 % of an R-MAT's edges), their
 //                         contributions live in shared memory where they are needed;
@@ -22,10 +22,10 @@
 //                         is summed from the window in stored order.  4 + 2 bytes per entry.
 //       K_S  pb_straddle  rows longer than a window: their per-bin partial sums added in bin order.
 //       K_F  pb_final     per row: the hub part sum_{v in H} contrib[v] through a shared-memory copy of
-//                         the hub contributions (u16 index per entry, 2 bytes), + the M part, new score,
-//                         error, new contribution.
+//                         the hub contributions (u16 index per entry, 2 bytes; a lane per row of at most 64
+//                         entries, the warp per longer row), + the M part, new score, error, new contribution.
 //     No atomics on floating point anywhere: sums have a fixed order, results are bit-reproducible.
-//   mode 0            the round-1 gather pull (one persistent launch, L2 eviction hints), kept for A/B runs.
+//   mode 0 (default)  the round-1 gather pull (one persistent launch, L2 eviction hints).
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -569,8 +569,7 @@ extern "C" int cozo_gpu_pagerank(cozo_gpu_graph_t* g, float damping, double tol,
   const uint32_t n = g->n;
   if (n == 0) return 0;  // pagerank.rs:43-45
   const DeviceInfo& di = device_info();
-  // default = the engine that has run on a GPU (round-1 gather pull); "pagerank.mode" = 1 selects propagation blocking,
-  // which is model-tested on the CPU but has not run on a device yet (gpurun closed mid-round, DESIGN.md §0)
+  // default = the round-1 gather pull; "pagerank.mode" = 1 selects propagation blocking (DESIGN.md §3.3)
   const int64_t mode = get_option("pagerank.mode", 0);
   uint32_t NH = (uint32_t)std::min<int64_t>(65536, std::max<int64_t>(0, get_option("pagerank.hub_slots", 16384)));
   NH &= ~3u;

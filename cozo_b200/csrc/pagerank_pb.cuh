@@ -1,7 +1,7 @@
 // pagerank_pb.cuh — device code of the propagation-blocking PageRank engine (pagerank.cu, mode 1): the staging
 // kernels and the bodies of the four per-iteration passes.  Kept in a header so that the SAME source is compiled by
 // nvcc into libcozo_gpu.so and, by tests/emu (a CPU SIMT emulator, test infrastructure), into a host program that runs
-// the passes thread for thread — the engine has not run on a GPU yet (DESIGN.md §0).
+// the passes thread for thread.
 #pragma once
 #include "common.cuh"
 
@@ -366,7 +366,22 @@ __device__ __forceinline__ void pb_final_body(const PbArgs& a, uint8_t* pb_smem)
       if (T <= KF_STAGE) {
         for (uint32_t i = lane; i < T; i += 32) stage[i] = a.hub_idx[gb + i];
         __syncwarp();
-        for (uint32_t j = h0 - gb; j < h1 - gb; ++j) s += hub[stage[j]];
+        // as in K_B: a lane sums a row of at most 64 entries, longer rows are summed by the whole warp (lanes strided,
+        // shuffle tree), so that no f32 chain is longer than 64 additions (a serial chain of 2048 equal terms drifts by
+        // about 2e-5 relative)
+        const uint32_t len = h1 - h0;
+        if (len <= 64)
+          for (uint32_t j = h0 - gb; j < h1 - gb; ++j) s += hub[stage[j]];
+        uint32_t lm = __ballot_sync(0xffffffffu, len > 64);
+        while (lm) {
+          const int l = __ffs(lm) - 1;
+          lm &= lm - 1;
+          const uint32_t ls = __shfl_sync(0xffffffffu, h0, l) - gb, le = __shfl_sync(0xffffffffu, h1, l) - gb;
+          float p = 0.f;
+          for (uint32_t j = ls + lane; j < le; j += 32) p += hub[stage[j]];
+          p = warp_sum(p);
+          if (lane == l) s = p;
+        }
         __syncwarp();
       } else {
         for (uint32_t l = 0; l < nvalid; ++l) {  // long hub lists: the warp sums one row at a time

@@ -1,16 +1,17 @@
 """GPU tests of code that has NOT run on a device yet.
 
 gpurun was closed mid-round (three boxes were lost under long calls while the pod was draining), after these
-features were written but before they could be run: the propagation-blocking PageRank engine (pagerank.mode=1), the
-compacted-frontier and wide SSSP forms (sssp.frontier / sssp.wide), the zero-weight-cycle refusal of betweenness, the
-builder's fidelity mode (batches of one) and extend_candidates.  All of them are off by default (or, for the builder
+features were written but before they could be run: the compacted-frontier and wide SSSP forms (sssp.frontier /
+sssp.wide), the zero-weight-cycle refusal of betweenness, the builder's fidelity mode (batches of one) and
+extend_candidates.  The propagation-blocking PageRank engine (pagerank.mode=1) has since run on the H100; its tests are
+in tests/test_graph_gpu.py and tests/test_pagerank_exact_gpu.py.  All of them are off by default (or, for the builder
 modes, only reached through explicit arguments).  The tests carry the marker `gpu_unverified` instead of `gpu`, so the
 round-end `pytest -m gpu` does not select them, and they skip unless COZO_RUN_UNVERIFIED=1 is set:
 
     COZO_RUN_UNVERIFIED=1 python -m pytest tests/test_unverified_gpu.py -q
 
-The layout logic of the PageRank engine is additionally covered on the CPU by tests/test_pagerank_model_cpu.py, and this
-whole file passes (12 / 12) against the CPU-emulated build of the library (tests/test_emu_lib_cpu.py; record in
+This whole file passed (12 / 12, with the PageRank engine test then still in it) against the CPU-emulated build of the
+library (tests/test_emu_lib_cpu.py; record in
 profiles/r02_emu_gpu_testfiles.txt) — which is how the extend_candidates interleaving bug was found and fixed.
 """
 import os
@@ -24,56 +25,6 @@ from tests.util import recall, rmat_edges, uniform_vectors
 
 pytestmark = [pytest.mark.gpu_unverified,
               pytest.mark.skipif(os.environ.get("COZO_RUN_UNVERIFIED") != "1", reason="not yet run on a GPU; opt in with COZO_RUN_UNVERIFIED=1")]
-
-
-PR_DEFAULTS = {"pagerank.mode": 1, "pagerank.hub_slots": 16384, "pagerank.group_slots": 32768, "pagerank.window": 24576,
-               "pagerank.chunk": 262144}
-PR_ENGINES = [
-    {"pagerank.mode": 0},                                                      # round-1 gather pull
-    {},                                                                        # propagation blocking, defaults
-    {"pagerank.hub_slots": 64, "pagerank.group_slots": 256, "pagerank.window": 512, "pagerank.chunk": 1024},
-    {"pagerank.hub_slots": 0, "pagerank.group_slots": 64, "pagerank.window": 64},          # no hub table, tiny tiles
-    {"pagerank.hub_slots": 1024, "pagerank.group_slots": 4096, "pagerank.window": 3001},   # odd window
-]
-
-
-@pytest.mark.parametrize("engine", range(len(PR_ENGINES)))
-def test_pagerank_engines_and_blockings(gpu, engine):
-    """every engine / blocking geometry computes the same iteration: <= 1e-5 of the oracle on R-MAT (all code paths of
-    the blocking: several groups, many bins, rows that straddle windows, empty rows), bit-identical reruns"""
-    opts = {**PR_DEFAULTS, **PR_ENGINES[engine]}
-    try:
-        for k, v in opts.items():
-            gpu.set_option(k, v)
-        for scale, iters in ((13, 6), (9, 4)):
-            n, src, dst = rmat_edges(scale, 16, 0x5EED0004 + scale)
-            g = gpu.Graph(n, src, dst)
-            os_, oit, oerr = O.OracleGraph(n, src, dst).pagerank(0.85, 0.0, iters, variant="jacobi", n_threads=8)
-            gs, git, gerr, _ = g.pagerank(0.85, 0.0, iters)
-            assert git == oit and np.max(np.abs(gs - os_) / os_) <= 1e-5
-            assert abs(gerr - oerr) <= 0.02 * oerr + 1e-6
-            assert np.array_equal(gs, g.pagerank(0.85, 0.0, iters)[0])
-        # a star: one row with 4999 in-edges (many windows long at the small geometries) + reverse edges
-        n = 5000
-        src = np.concatenate([np.arange(1, n), np.zeros(n - 1)]).astype(np.uint32)
-        dst = np.concatenate([np.zeros(n - 1), np.arange(1, n)]).astype(np.uint32)
-        gs = gpu.Graph(n, src, dst).pagerank(0.85, 0.0, 5)[0]
-        s64 = np.full(n, 1.0 / n)
-        outdeg = np.bincount(src, minlength=n).astype(np.float64)
-        for _ in range(5):
-            nxt = np.full(n, 0.15 / n)
-            np.add.at(nxt, dst, 0.85 * (s64 / outdeg)[src])
-            s64 = nxt
-        assert np.max(np.abs(gs - s64) / s64) <= 4e-6
-        # a path graph and a graph whose last ids have no edges at all
-        src = np.arange(0, 300, dtype=np.uint32)
-        dst = src + 1
-        g = gpu.Graph(1000, src, dst)
-        os_, _, _ = O.OracleGraph(1000, src, dst).pagerank(0.85, 0.0, 7)
-        assert np.allclose(g.pagerank(0.85, 0.0, 7)[0], os_, rtol=1e-6)
-    finally:
-        for k, v in PR_DEFAULTS.items():
-            gpu.set_option(k, v)
 
 
 def test_sssp_queue_frontier_and_large_graph(gpu):
