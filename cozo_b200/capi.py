@@ -26,7 +26,7 @@ EXPORTS = [
     "cozo_gpu_hnsw_search_dev", "cozo_gpu_hnsw_search_scatter_dev", "cozo_gpu_hnsw_build", "cozo_gpu_hnsw_insert", "cozo_gpu_hnsw_insert_at", "cozo_gpu_hnsw_remove", "cozo_gpu_hnsw_compact", "cozo_gpu_hnsw_update", "cozo_gpu_hnsw_info", "cozo_gpu_hnsw_level_size",
     "cozo_gpu_hnsw_export_level", "cozo_gpu_hnsw_export_level_dist", "cozo_gpu_hnsw_export_live", "cozo_gpu_hnsw_vectors_dev", "cozo_gpu_topk_merge_dev", "cozo_gpu_graph_stage",
     "cozo_gpu_graph_free", "cozo_gpu_graph_export", "cozo_gpu_pagerank", "cozo_gpu_sssp_multi", "cozo_gpu_closeness",
-    "cozo_gpu_betweenness", "cozo_gpu_clustering", "cozo_gpu_sssp_paths",
+    "cozo_gpu_betweenness", "cozo_gpu_clustering", "cozo_gpu_sssp_paths", "cozo_gpu_sssp_goals",
     "cozo_gpu_shards_unique_id", "cozo_gpu_shards_init", "cozo_gpu_shards_free", "cozo_gpu_shards_info",
     "cozo_gpu_hnsw_stage_sharded", "cozo_gpu_hnsw_search_sharded", "cozo_gpu_hnsw_search_sharded_dev",
     "cozo_gpu_hnsw_search_filtered", "cozo_gpu_hnsw_search_filtered_dev", "cozo_gpu_hnsw_search_f64",
@@ -116,6 +116,7 @@ def load():
     L.cozo_gpu_betweenness.argtypes = [vp, vp, vp, vp]
     L.cozo_gpu_clustering.argtypes = [vp, vp, vp, vp, vp, vp]
     L.cozo_gpu_sssp_paths.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp]
+    L.cozo_gpu_sssp_goals.argtypes = [vp, vp, u32, vp, u32, C.c_int32, vp, vp, vp, u64, vp, vp, u64, vp, vp]
     L.cozo_gpu_hnsw_search_filtered.argtypes = [vp, vp, u32, u32, u32, f64, vp, vp, vp, vp, C.POINTER(SearchStats)]
     L.cozo_gpu_hnsw_search_filtered_dev.argtypes = [vp, vp, u32, u32, u32, f64, vp, vp, vp, vp, vp, vp]
     L.cozo_gpu_hnsw_search_f64.argtypes = [vp, vp, u32, u32, u32, f64, vp, vp, vp, vp, C.POINTER(SearchStats)]
@@ -599,6 +600,34 @@ class Graph:
                 break
             max_len = int(ln.max())
         return [(float(cost[i]), paths[i, :ln[i]].tolist()) for i in range(k)], ms.value
+
+    def sssp_goals(self, sources, goals, keep_ties=False, poison=None, cap=None):
+        """shortest paths from every source to the goals only; each search stops once its goals are settled.
+        -> (costs f32 [n_src, n_goals], rows, kernel ms).  rows: without keep_ties, per pair (si, gi) the path list
+        start..goal ([] when unreachable), as a list of n_src lists; with keep_ties, per source the tied-predecessor
+        edges leading back from its goals, a u32 array [k, 2] of (v, p).  The first call has room for `cap` path nodes
+        or tie edges (default: 64 per pair) and is repeated with the reported total when that is too small."""
+        sources = np.ascontiguousarray(sources, np.uint32)
+        goals = np.ascontiguousarray(goals, np.uint32)
+        ns, ng = sources.size, goals.size
+        cap = 64 * ns * ng if cap is None else int(cap)
+        while True:
+            cost = np.zeros((ns, ng), np.float32)
+            off = np.zeros((ns + 1) if keep_ties else (ns * ng + 1), np.uint64)
+            rows = np.zeros(max(cap, 1) * (2 if keep_ties else 1), np.uint32)
+            ms = C.c_double()
+            args = (None, None, 0, _p(off), _p(rows), cap) if keep_ties else (_p(off), _p(rows), cap, None, None, 0)
+            _check(load().cozo_gpu_sssp_goals(self._h, _p(sources), ns, _p(goals), ng, int(bool(keep_ties)), _p(cost),
+                                              *args, C.byref(ms), _p(poison)))
+            if int(off[-1]) <= cap:
+                break
+            cap = int(off[-1])
+        off = off.astype(np.int64)
+        if keep_ties:
+            edges = rows[:2 * off[-1]].reshape(-1, 2)
+            return cost, [edges[off[i]:off[i + 1]] for i in range(ns)], ms.value
+        paths = [rows[off[i]:off[i + 1]].tolist() for i in range(ns * ng)]
+        return cost, [paths[i * ng:(i + 1) * ng] for i in range(ns)], ms.value
 
     def clustering(self, poison=None):
         cc = np.zeros(self.n, np.float64)

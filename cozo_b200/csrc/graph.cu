@@ -69,15 +69,33 @@ __global__ void __launch_bounds__(256) sssp_kernel(const uint32_t* __restrict__ 
   sssp_body<FORB, SMEM>(out_ptr, out_idx, out_w, n, sources, n_src, state, flags, flags_stride, fs, sssp_smem);
 }
 
+// the same search stopping once every goal is settled (cozo_gpu_sssp_goals); no forbidden sets
+template <bool SMEM>
+__global__ void __launch_bounds__(256) sssp_goal_kernel(const uint32_t* __restrict__ out_ptr,
+                                                        const uint32_t* __restrict__ out_idx,
+                                                        const float* __restrict__ out_w, uint32_t n,
+                                                        const uint32_t* __restrict__ sources, uint32_t n_src,
+                                                        unsigned long long* state, uint8_t* flags, size_t flags_stride,
+                                                        GoalSet gs) {
+  extern __shared__ __align__(16) uint8_t sssp_smem[];
+  __shared__ float red[64];
+  gs.red = red;
+  sssp_body<false, SMEM, true>(out_ptr, out_idx, out_w, n, sources, n_src, state, flags, flags_stride, ForbiddenSets{},
+                               sssp_smem, gs);
+}
+
 // launch helper.  Default = the flag-scan kernel (shared-memory state when it fits).  Options, both off by default
 // because neither form has run on a GPU yet: "sssp.frontier" = 1 -> compacted frontier queues (one CTA per source),
 // "sssp.wide" = 1 -> many CTAs per source with one launch per round (host loop, capped at n + 2 rounds).
 // "sssp.smem" = 0 keeps the flag-scan state in HBM even when it fits shared memory, so that tests reach the form every
 // graph above ~23 k nodes takes with graphs small enough for exact references.
+// Goals (gs.goals != nullptr, FORB = false): the flag-scan form stops once they are settled; the other two forms run to
+// the fixed point, which gives the same answers.
 static size_t sssp_flags_stride(uint32_t n) { return ((size_t)n * 9 + 15) & ~(size_t)15; }
 template <bool FORB>
 static cudaError_t launch_sssp(cozo_gpu_graph_t* g, const uint32_t* d_sources, uint32_t n_src,
-                               unsigned long long* state, uint8_t* flags, ForbiddenSets fs, cudaStream_t st) {
+                               unsigned long long* state, uint8_t* flags, ForbiddenSets fs, cudaStream_t st,
+                               GoalSet gs = GoalSet{}) {
   const uint32_t n = g->n;
   const size_t need = (size_t)n * 10;
   const DeviceInfo& di = device_info();
@@ -115,17 +133,26 @@ static cudaError_t launch_sssp(cozo_gpu_graph_t* g, const uint32_t* d_sources, u
   if (need + 1024 <= di.smem_optin && get_option("sssp.smem", 1) != 0) {
     // raise the kernel's dynamic shared-memory limit, never lower it (concurrent callers with other graphs)
     static std::mutex mu;
-    static size_t raised[2] = {0, 0};
+    static size_t raised[3] = {0, 0, 0};
+    const int slot = gs.goals ? 2 : FORB ? 1 : 0;
     {
       std::lock_guard<std::mutex> lk(mu);
-      if (need > raised[FORB ? 1 : 0]) {
-        cudaError_t e = cudaFuncSetAttribute(sssp_kernel<FORB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need);
+      if (need > raised[slot]) {
+        cudaError_t e = gs.goals ? cudaFuncSetAttribute(sssp_goal_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need)
+                                 : cudaFuncSetAttribute(sssp_kernel<FORB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need);
         if (e != cudaSuccess) return e;
-        raised[FORB ? 1 : 0] = need;
+        raised[slot] = need;
       }
     }
-    sssp_kernel<FORB, true><<<n_src, 256, need, st>>>(g->out_ptr, g->out_idx, g->out_w, n, d_sources, n_src, state, flags,
-                                                      fstride, fs);
+    if (gs.goals)
+      sssp_goal_kernel<true><<<n_src, 256, need, st>>>(g->out_ptr, g->out_idx, g->out_w, n, d_sources, n_src, state, flags,
+                                                       fstride, gs);
+    else
+      sssp_kernel<FORB, true><<<n_src, 256, need, st>>>(g->out_ptr, g->out_idx, g->out_w, n, d_sources, n_src, state, flags,
+                                                        fstride, fs);
+  } else if (gs.goals) {
+    sssp_goal_kernel<false><<<n_src, 256, 0, st>>>(g->out_ptr, g->out_idx, g->out_w, n, d_sources, n_src, state, flags,
+                                                   fstride, gs);
   } else {
     sssp_kernel<FORB, false><<<n_src, 256, 0, st>>>(g->out_ptr, g->out_idx, g->out_w, n, d_sources, n_src, state, flags,
                                                     fstride, fs);
@@ -287,7 +314,7 @@ namespace cozo {
 // caps a chunk at k sources, so that tests run several chunks on small graphs.
 template <class PerChunk>
 static int sssp_chunks(cozo_gpu_graph_t* g, CallStream& cs, const uint32_t* sources_host, uint32_t n_src,
-                       size_t extra_per_src, const volatile int* poison, PerChunk per_chunk) {
+                       size_t extra_per_src, const volatile int* poison, PerChunk per_chunk, GoalSet gs = GoalSet{}) {
   const uint32_t n = g->n;
   const size_t fstride = sssp_flags_stride(n);
   const size_t per_src = (size_t)n * 8 + fstride + extra_per_src;
@@ -310,7 +337,7 @@ static int sssp_chunks(cozo_gpu_graph_t* g, CallStream& cs, const uint32_t* sour
     uint32_t c = std::min(chunk, n_src - s0);
     cudaMemcpyAsync(dsrc.p, sources_host + s0, (size_t)c * 4, cudaMemcpyHostToDevice, cs.s);
     cudaError_t le = launch_sssp<false>(g, dsrc.as<uint32_t>(), c, state.as<unsigned long long>(), flags.as<uint8_t>(),
-                                        ForbiddenSets{}, cs.s);
+                                        ForbiddenSets{}, cs.s, gs);
     if (le != cudaSuccess) {
       ret = set_error(COZO_GPU_ECUDA, "sssp launch failed: %s", cudaGetErrorString(le));
       break;
@@ -351,6 +378,101 @@ extern "C" int cozo_gpu_sssp_multi(cozo_gpu_graph_t* g, const uint32_t* sources,
                        COZO_CUDA(cudaMemcpyAsync(out_pred + (size_t)s0 * n, dp.p, total * 4, cudaMemcpyDeviceToHost, cs.s));
                      return 0;
                    });
+  const double ms = cs.stop();
+  if (out_kernel_ms) *out_kernel_ms = ms;
+  return rc;
+}
+
+extern "C" int cozo_gpu_sssp_goals(cozo_gpu_graph_t* g, const uint32_t* sources, uint32_t n_src, const uint32_t* goals,
+                                   uint32_t n_goals, int32_t keep_ties, float* out_cost, uint64_t* out_path_off,
+                                   uint32_t* out_paths, uint64_t paths_cap, uint64_t* out_tie_off,
+                                   uint32_t* out_tie_edges, uint64_t ties_cap, double* out_kernel_ms,
+                                   const volatile int* poison) {
+  const uint64_t pairs = (uint64_t)n_src * n_goals;
+  uint64_t* off_out = keep_ties ? out_tie_off : out_path_off;
+  uint32_t* rows_out = keep_ties ? out_tie_edges : out_paths;
+  const uint64_t cap = keep_ties ? ties_cap : paths_cap;
+  if (!g || (n_src && !sources) || (n_goals && !goals) || (pairs && !out_cost) || !off_out || (cap && !rows_out))
+    return set_error(COZO_GPU_EINVAL, "null argument");
+  int rc = ensure_init();
+  if (rc) return rc;
+  if (out_kernel_ms) *out_kernel_ms = 0;
+  const uint32_t n = g->n;
+  for (uint32_t i = 0; i < n_src; ++i)
+    if (sources[i] >= n) return set_error(COZO_GPU_EINVAL, "source %u out of range", sources[i]);
+  {
+    std::vector<uint32_t> sorted(goals, goals + n_goals);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint32_t i = 0; i < n_goals; ++i) {
+      if (sorted[i] >= n) return set_error(COZO_GPU_EINVAL, "goal %u out of range", sorted[i]);
+      if (i && sorted[i] == sorted[i - 1]) return set_error(COZO_GPU_EINVAL, "goal %u given twice", sorted[i]);
+    }
+  }
+  // offsets per pair (paths) or per source (tied edges); a source with no goals has none of either
+  const uint64_t n_off = keep_ties ? (uint64_t)n_src + 1 : pairs + 1;
+  std::fill(off_out, off_out + n_off, 0);
+  if (pairs == 0) return 0;
+  CallStream cs;
+  rc = cs.init();
+  if (rc) return rc;
+  DevBuf dgoal, dcost, dscan, dmark, drows, tmp;
+  COZO_CUDA(cudaMalloc(&dgoal.p, (size_t)n_goals * 4));
+  COZO_CUDA(cudaMemcpyAsync(dgoal.p, goals, (size_t)n_goals * 4, cudaMemcpyHostToDevice, cs.s));
+  const GoalSet gs{dgoal.as<uint32_t>(), n_goals, nullptr};
+  uint64_t base = 0, rows_cap = 0;  // rows so far; capacity of drows in rows (a path node, or one (v, p) pair)
+  bool fits = true;
+  size_t tmp_bytes = 0;
+  rc = sssp_chunks(
+      g, cs, sources, n_src, (size_t)n_goals * 12 + (keep_ties ? (size_t)n + 8 : 0), poison,
+      [&](uint32_t s0, uint32_t c, unsigned long long* state, uint32_t* dsrc) -> int {
+        const uint64_t pc = (uint64_t)c * n_goals;
+        const uint64_t m = keep_ties ? (uint64_t)c : pc;  // entries scanned, plus the one that receives the total
+        if (!dcost.p) {  // the first chunk is the largest
+          COZO_CUDA(cudaMalloc(&dcost.p, pc * 4));
+          COZO_CUDA(cudaMalloc(&dscan.p, (m + 1) * 8));
+          if (keep_ties) COZO_CUDA(cudaMalloc(&dmark.p, (size_t)c * n));
+          cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, dscan.as<uint64_t>(), dscan.as<uint64_t>(), (int64_t)m + 1,
+                                        cs.s);
+          COZO_CUDA(cudaMalloc(&tmp.p, std::max<size_t>(tmp_bytes, 16)));
+        }
+        uint64_t* scan = dscan.as<uint64_t>();
+        sssp_goal_len_kernel<<<(uint32_t)((pc + 256) / 256), 256, 0, cs.s>>>(state, n, dsrc, gs.goals, n_goals, c,
+                                                                            dcost.as<float>(), keep_ties ? nullptr : scan);
+        if (keep_ties)
+          sssp_tie_mark_kernel<<<c, 256, 0, cs.s>>>(g->out_ptr, g->out_idx, g->out_w, n, dsrc, gs, c, state,
+                                                   dmark.as<uint8_t>(), scan);
+        size_t t3 = tmp_bytes;
+        cub::DeviceScan::ExclusiveSum(tmp.p, t3, scan, scan, (int64_t)m + 1, cs.s);
+        COZO_CUDA(cudaGetLastError());
+        COZO_CUDA(cudaMemcpyAsync(out_cost + (size_t)s0 * n_goals, dcost.p, pc * 4, cudaMemcpyDeviceToHost, cs.s));
+        uint64_t* off = off_out + (keep_ties ? (uint64_t)s0 : (uint64_t)s0 * n_goals);
+        COZO_CUDA(cudaMemcpyAsync(off, scan, (m + 1) * 8, cudaMemcpyDeviceToHost, cs.s));
+        COZO_CUDA(cudaStreamSynchronize(cs.s));
+        const uint64_t total = off[m];
+        for (uint64_t i = 0; i <= m; ++i) off[i] += base;
+        fits = fits && base + total <= cap;
+        if (fits && total) {
+          if (rows_cap < total) {
+            if (drows.p) cudaFree(drows.p);
+            drows.p = nullptr;
+            COZO_CUDA(cudaMalloc(&drows.p, total * (keep_ties ? 8 : 4)));
+            rows_cap = total;
+          }
+          if (keep_ties)
+            sssp_tie_write_kernel<<<c, 256, 0, cs.s>>>(g->out_ptr, g->out_idx, g->out_w, n, dsrc, c, state,
+                                                      dmark.as<uint8_t>(), scan, drows.as<uint32_t>());
+          else
+            sssp_goal_path_kernel<<<(uint32_t)((pc + 255) / 256), 256, 0, cs.s>>>(state, n, gs.goals, n_goals, c, scan,
+                                                                                 drows.as<uint32_t>());
+          COZO_CUDA(cudaGetLastError());
+          const uint64_t per_row = keep_ties ? 2 : 1;
+          COZO_CUDA(cudaMemcpyAsync(rows_out + base * per_row, drows.p, total * per_row * 4, cudaMemcpyDeviceToHost,
+                                    cs.s));
+        }
+        base += total;
+        return 0;
+      },
+      gs);
   const double ms = cs.stop();
   if (out_kernel_ms) *out_kernel_ms = ms;
   return rc;

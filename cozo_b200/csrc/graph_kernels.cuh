@@ -23,16 +23,30 @@ struct ForbiddenSets {
   const uint32_t *fn_ptr, *fn_nodes, *fe_ptr, *fe_src, *fe_dst;
 };
 
+// The goals a search may stop at (cozo_gpu_sssp_goals): distinct node ids, shared by every source.
+// `red` = 64 floats of shared memory for the per-warp lower bounds and largest goal distances of a round.
+struct GoalSet {
+  const uint32_t* goals;
+  uint32_t n;
+  float* red;
+};
+
 // SMEM = the per-source state (8 B/node) and the two frontier flag arrays (1 B/node each) live in
 // shared memory (graphs up to ~22 k nodes); the final state is copied out for the read-out kernels.
 // A warp takes one frontier node at a time and its lanes stride the node's out-edges.  A round scans the
 // flag arrays (O(n) per round): the default form, verified on the GPU since round 1.
-template <bool FORB, bool SMEM>
+//
+// GOALS = stop once every goal is settled.  L = the smallest distance written by a successful CAS in the round is a
+// lower bound on every node of the next frontier, and every later update is >= L (weights are non-negative and
+// fl32(a + w) >= a).  So when every goal is finite and L > G = max goal distance, no node at distance <= G can change
+// again: the goals' costs, their predecessor paths and every tied predecessor of a node at distance <= G are those of
+// the full run.  The test is strict: with L == G a zero-weight edge could still bring a new tied predecessor at G.
+template <bool FORB, bool SMEM, bool GOALS = false>
 __device__ __forceinline__ void sssp_body(const uint32_t* __restrict__ out_ptr, const uint32_t* __restrict__ out_idx,
                                           const float* __restrict__ out_w, uint32_t n,
                                           const uint32_t* __restrict__ sources, uint32_t n_src,
                                           unsigned long long* state, uint8_t* flags, size_t flags_stride,
-                                          ForbiddenSets fs, uint8_t* sssp_smem) {
+                                          ForbiddenSets fs, uint8_t* sssp_smem, GoalSet gs = GoalSet{}) {
   const uint32_t si = blockIdx.x;
   if (si >= n_src) return;
   uint32_t fnb = 0, fne = 0, feb = 0, fee = 0;
@@ -65,6 +79,7 @@ __device__ __forceinline__ void sssp_body(const uint32_t* __restrict__ out_ptr, 
     if (threadIdx.x == 0) s_any = 0;
     __syncthreads();
     bool any_local = false;
+    float lb = __int_as_float(0x7f800000);  // GOALS: smallest distance this thread wrote in the round
     for (uint32_t u = warp; u < n; u += nwarps) {
       if (!cur[u]) continue;  // warp-uniform
       __syncwarp();
@@ -87,17 +102,39 @@ __device__ __forceinline__ void sssp_body(const uint32_t* __restrict__ out_ptr, 
           if (got == old) {
             nxt[v] = 1;
             any_local = true;
+            if constexpr (GOALS) lb = fminf(lb, nd);
             break;
           }
           old = got;
         }
       }
     }
+    if constexpr (GOALS) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) lb = fminf(lb, __shfl_xor_sync(0xffffffffu, lb, o));
+      if (lane == 0) gs.red[warp] = lb;
+    }
     if (any_local) s_any = 1;
     __syncthreads();
     const int any = s_any;
+    if constexpr (GOALS) {  // this round's writes are complete: the largest goal distance, +inf while a goal is unreached
+      float gmax = 0.0f;
+      for (uint32_t i = threadIdx.x; i < gs.n; i += blockDim.x)
+        gmax = fmaxf(gmax, __uint_as_float((uint32_t)(st[gs.goals[i]] >> 32)));
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) gmax = fmaxf(gmax, __shfl_xor_sync(0xffffffffu, gmax, o));
+      if (lane == 0) gs.red[32 + warp] = gmax;
+    }
     __syncthreads();
     if (!any) break;
+    if constexpr (GOALS) {
+      float L = gs.red[0], G = gs.red[32];
+      for (uint32_t w = 1; w < nwarps; ++w) {
+        L = fminf(L, gs.red[w]);
+        G = fmaxf(G, gs.red[32 + w]);
+      }
+      if (G < L) break;  // G finite: L is +inf only when no update can follow
+    }
     uint8_t* t = cur;
     cur = nxt;
     nxt = t;
@@ -315,6 +352,144 @@ __global__ void sssp_path_kernel(const unsigned long long* state, uint32_t n, co
   for (uint32_t i = cnt; i-- > 0;) {
     p[i] = cur;
     cur = (uint32_t)(st[cur] & 0xFFFFFFFFull);
+  }
+}
+
+// ---- cozo_gpu_sssp_goals read-out: pair i = si * n_goals + gi of a chunk ----
+// cost of every pair and, when `len` is given, its path length in nodes (0 when unreachable); len[c * n_goals] = 0 so
+// that an exclusive scan over c * n_goals + 1 entries leaves the chunk's total in the last one
+__global__ void sssp_goal_len_kernel(const unsigned long long* state, uint32_t n, const uint32_t* sources,
+                                     const uint32_t* goals, uint32_t n_goals, uint32_t c, float* cost, uint64_t* len) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const uint64_t pairs = (uint64_t)c * n_goals;
+  if (len && i == pairs) len[i] = 0;
+  if (i >= pairs) return;
+  const uint32_t si = (uint32_t)(i / n_goals);
+  const unsigned long long* st = state + (size_t)si * n;
+  const uint32_t s = sources[si], t = goals[i % n_goals];
+  const float d = __uint_as_float((uint32_t)(st[t] >> 32));
+  cost[i] = d;
+  if (!len) return;
+  uint64_t cnt = 0;
+  if (isfinite(d)) {
+    uint32_t cur = t;
+    for (cnt = 1; cur != s && cnt <= n; ++cnt) cur = (uint32_t)(st[cur] & 0xFFFFFFFFull);
+  }
+  len[i] = cnt;
+}
+
+// path of pair i at paths[off[i] .. off[i+1]), start..goal
+__global__ void sssp_goal_path_kernel(const unsigned long long* state, uint32_t n, const uint32_t* goals,
+                                      uint32_t n_goals, uint32_t c, const uint64_t* off, uint32_t* paths) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (uint64_t)c * n_goals) return;
+  const unsigned long long* st = state + (size_t)(i / n_goals) * n;
+  uint32_t cur = goals[i % n_goals];
+  for (uint64_t k = off[i + 1]; k-- > off[i];) {
+    paths[k] = cur;
+    cur = (uint32_t)(st[cur] & 0xFFFFFFFFull);
+  }
+}
+
+// keep_ties: the tied-predecessor edges that lead back from the goals of one source (one CTA per source).
+// C = the goals with a finite cost other than s, closed under "p has a tight edge (p -> v) with v in C, v != s";
+// E = those tight edges, one per CSR edge.  Marking is idempotent, so the closure ends on zero-weight tied cycles too.
+// The out-CSR is scanned in rounds (the staged in-CSR carries no weights), as betweenness_kernel walks its tie DAG.
+__device__ __forceinline__ bool tie_edge(const unsigned long long* st, const uint8_t* mark, uint32_t s, float du,
+                                         uint32_t v, float w) {
+  return v != s && mark[v] && du + w == __uint_as_float((uint32_t)(st[v] >> 32));
+}
+
+__global__ void __launch_bounds__(256) sssp_tie_mark_kernel(const uint32_t* __restrict__ out_ptr,
+                                                            const uint32_t* __restrict__ out_idx,
+                                                            const float* __restrict__ out_w, uint32_t n,
+                                                            const uint32_t* __restrict__ sources, GoalSet gs, uint32_t c,
+                                                            const unsigned long long* state, uint8_t* mark_buf,
+                                                            uint64_t* count) {
+  const uint32_t si = blockIdx.x;
+  if (si >= c) return;
+  const unsigned long long* st = state + (size_t)si * n;
+  uint8_t* mark = mark_buf + (size_t)si * n;
+  const uint32_t s = sources[si];
+  const int lane = threadIdx.x & 31;
+  const uint32_t warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  __shared__ int s_any;
+  __shared__ unsigned long long s_cnt[32];
+  for (uint32_t v = threadIdx.x; v < n; v += blockDim.x) mark[v] = 0;
+  __syncthreads();
+  for (uint32_t i = threadIdx.x; i < gs.n; i += blockDim.x) {
+    const uint32_t t = gs.goals[i];
+    if (t != s && isfinite(__uint_as_float((uint32_t)(st[t] >> 32)))) mark[t] = 1;
+  }
+  for (;;) {
+    if (threadIdx.x == 0) s_any = 0;
+    __syncthreads();
+    bool any_local = false;
+    for (uint32_t u = warp; u < n; u += nwarps) {
+      if (mark[u]) continue;  // warp-uniform: read before any lane of this warp can set it
+      const float du = __uint_as_float((uint32_t)(st[u] >> 32));
+      if (!isfinite(du)) continue;
+      bool hit = false;
+      for (uint32_t k = out_ptr[u] + lane; k < out_ptr[u + 1] && !hit; k += 32)
+        hit = tie_edge(st, mark, s, du, out_idx[k], out_w ? out_w[k] : 1.0f);
+      if (__ballot_sync(0xffffffffu, hit)) {
+        if (lane == 0) mark[u] = 1;
+        any_local = true;
+      }
+      __syncwarp();
+    }
+    if (any_local) s_any = 1;
+    __syncthreads();
+    const int any = s_any;
+    __syncthreads();
+    if (!any) break;
+  }
+  unsigned long long cnt = 0;
+  for (uint32_t u = warp; u < n; u += nwarps) {
+    const float du = __uint_as_float((uint32_t)(st[u] >> 32));
+    if (!mark[u] || !isfinite(du)) continue;  // a tight edge into C starts in C
+    for (uint32_t k = out_ptr[u] + lane; k < out_ptr[u + 1]; k += 32)
+      cnt += tie_edge(st, mark, s, du, out_idx[k], out_w ? out_w[k] : 1.0f) ? 1ull : 0ull;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if (lane == 0) s_cnt[warp] = cnt;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long t = 0;
+    for (uint32_t w = 0; w < nwarps; ++w) t += s_cnt[w];
+    count[si] = t;
+    if (si == c - 1) count[c] = 0;  // scanned over c + 1 entries: the chunk's total lands in the last
+  }
+}
+
+// the edges counted above as (v, p) pairs at edges[2 * off[si] ...], in no particular order within a source
+__global__ void __launch_bounds__(256) sssp_tie_write_kernel(const uint32_t* __restrict__ out_ptr,
+                                                             const uint32_t* __restrict__ out_idx,
+                                                             const float* __restrict__ out_w, uint32_t n,
+                                                             const uint32_t* __restrict__ sources, uint32_t c,
+                                                             const unsigned long long* state, const uint8_t* mark_buf,
+                                                             const uint64_t* off, uint32_t* edges) {
+  const uint32_t si = blockIdx.x;
+  if (si >= c) return;
+  const unsigned long long* st = state + (size_t)si * n;
+  const uint8_t* mark = mark_buf + (size_t)si * n;
+  const uint32_t s = sources[si];
+  const int lane = threadIdx.x & 31;
+  const uint32_t warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  __shared__ unsigned long long s_at;
+  if (threadIdx.x == 0) s_at = off[si];
+  __syncthreads();
+  for (uint32_t u = warp; u < n; u += nwarps) {
+    const float du = __uint_as_float((uint32_t)(st[u] >> 32));
+    if (!mark[u] || !isfinite(du)) continue;
+    for (uint32_t k = out_ptr[u] + lane; k < out_ptr[u + 1]; k += 32) {
+      const uint32_t v = out_idx[k];
+      if (!tie_edge(st, mark, s, du, v, out_w ? out_w[k] : 1.0f)) continue;
+      const unsigned long long at = atomicAdd(&s_at, 1ull);
+      edges[2 * at] = v;
+      edges[2 * at + 1] = u;
+    }
   }
 }
 

@@ -313,21 +313,21 @@ struct PageRank : FixedRule {
 struct ShortestPathDijkstra : FixedRule {
   size_t arity(const Options&, const std::vector<std::string>&) const override { return 4; }
 
-  // every tied shortest path start -> target from the distances (the reference keeps
-  // predecessor lists while searching, :372-380, and enumerates them at :397-426)
-  static void collect(const StagedGraph& g, const std::vector<std::vector<std::pair<uint32_t, float>>>& in_edges,
-                      const float* dist, uint32_t start, std::vector<uint32_t>& chain,
-                      std::vector<std::vector<uint32_t>>& paths, const Poison& poison) {
-    uint32_t last = chain.back();
-    for (auto& e : in_edges[last]) {
-      uint32_t p = e.first;
-      if (!std::isfinite(dist[p]) || (float)(dist[p] + e.second) != dist[last]) continue;
+  // every tied shortest path start -> target over the tied-predecessor edges of one source (cozo_gpu_sssp_goals with
+  // keep_ties; the reference keeps predecessor lists while searching, :372-380, and enumerates them at :397-426).
+  // `tied` = (v, p) pairs sorted by v.
+  static void collect(const std::vector<std::pair<uint32_t, uint32_t>>& tied, uint32_t start,
+                      std::vector<uint32_t>& chain, std::vector<std::vector<uint32_t>>& paths, const Poison& poison) {
+    const uint32_t last = chain.back();
+    auto it = std::lower_bound(tied.begin(), tied.end(), std::make_pair(last, 0u));
+    for (; it != tied.end() && it->first == last; ++it) {
+      const uint32_t p = it->second;
       poison.check();
       chain.push_back(p);
       if (p == start) {
         paths.emplace_back(chain.rbegin(), chain.rend());
       } else {
-        collect(g, in_edges, dist, start, chain, paths, poison);
+        collect(tied, start, chain, paths, poison);
       }
       chain.pop_back();
     }
@@ -352,60 +352,77 @@ struct ShortestPathDijkstra : FixedRule {
     if (starting_nodes.empty()) return;
     const uint32_t n = g.node_count();
     std::vector<uint32_t> sources(starting_nodes.begin(), starting_nodes.end());
-    std::vector<float> dist((size_t)sources.size() * n);
-    std::vector<uint32_t> pred((size_t)sources.size() * n);
-    gpu_check(cozo_gpu_sssp_multi(g.g, sources.data(), (uint32_t)sources.size(), dist.data(), pred.data(), nullptr,
-                                  poison.raw()));
-    // keep_ties without a termination relation falls back to plain dijkstra (:85-87)
-    const bool ties = keep_ties && has_term;
-    std::vector<std::vector<std::pair<uint32_t, float>>> in_edges;
-    if (ties) {
-      std::vector<uint32_t> es, ed;
-      std::vector<float> ew;
-      g.edges(es, ed, ew);
-      in_edges.resize(n);
-      for (size_t e = 0; e < es.size(); ++e) in_edges[ed[e]].push_back({es[e], ew[e]});
+    auto put = [&](uint32_t start, uint32_t target, float cost, const uint32_t* path, size_t len) {
+      std::vector<DataValue> pl;
+      for (size_t i = 0; i < len; ++i) pl.push_back(g.indices[path[i]]);
+      out.put({g.indices[start], g.indices[target], DataValue::from_float((double)cost),
+               DataValue::from_list(std::move(pl))});  // :88-99
+    };
+    if (!has_term) {
+      // Goal for (): every node, 0..total (:233-235); keep_ties falls back to plain dijkstra (:85-87)
+      std::vector<float> dist((size_t)sources.size() * n);
+      std::vector<uint32_t> pred((size_t)sources.size() * n);
+      gpu_check(cozo_gpu_sssp_multi(g.g, sources.data(), (uint32_t)sources.size(), dist.data(), pred.data(), nullptr,
+                                    poison.raw()));
+      std::vector<uint32_t> path;
+      for (size_t si = 0; si < sources.size(); ++si) {
+        const uint32_t start = sources[si];
+        const float* d = dist.data() + si * n;
+        const uint32_t* p = pred.data() + si * n;
+        for (uint32_t t = 0; t < n; ++t) {
+          path.clear();
+          if (std::isfinite(d[t])) {  // :325-333; unreachable: (inf, []) :322-323
+            for (uint32_t cur = t; cur != start; cur = p[cur]) path.push_back(cur);
+            path.push_back(start);
+            std::reverse(path.begin(), path.end());
+          }
+          put(start, t, d[t], path.data(), path.size());
+        }
+        poison.check();
+      }
+      return;
     }
     // an empty termination set means "already exhausted": the search stops after the start
     // node and the goal iterator is empty (Goal for BTreeSet, :260-272) => no rows.
-    for (size_t si = 0; si < sources.size(); ++si) {
+    if (termination_nodes.empty()) return;
+    // with goals, each search stops once they are settled (is_exhausted, :312-315): only the goal answers come back
+    const std::vector<uint32_t> goals(termination_nodes.begin(), termination_nodes.end());
+    const size_t ns = sources.size(), ng = goals.size();
+    std::vector<float> cost(ns * ng);
+    std::vector<uint64_t> off(keep_ties ? ns + 1 : ns * ng + 1);
+    std::vector<uint32_t> rows;
+    for (uint64_t cap = 16 * ns * ng;;) {  // a first guess; the call reports the total when it does not fit
+      rows.resize(std::max<uint64_t>(cap, 1) * (keep_ties ? 2 : 1));
+      gpu_check(cozo_gpu_sssp_goals(g.g, sources.data(), (uint32_t)ns, goals.data(), (uint32_t)ng, keep_ties ? 1 : 0,
+                                    cost.data(), keep_ties ? nullptr : off.data(), keep_ties ? nullptr : rows.data(),
+                                    keep_ties ? 0 : cap, keep_ties ? off.data() : nullptr,
+                                    keep_ties ? rows.data() : nullptr, keep_ties ? cap : 0, nullptr, poison.raw()));
+      if (off.back() <= cap) break;
+      cap = off.back();
+    }
+    std::vector<std::pair<uint32_t, uint32_t>> tied;
+    std::vector<std::vector<uint32_t>> paths;
+    for (size_t si = 0; si < ns; ++si) {
       const uint32_t start = sources[si];
-      const float* d = dist.data() + si * n;
-      const uint32_t* p = pred.data() + si * n;
-      auto emit = [&](uint32_t target) {
-        float cost = d[target];
-        auto put = [&](const std::vector<uint32_t>& path) {
-          std::vector<DataValue> pl;
-          for (uint32_t u : path) pl.push_back(g.indices[u]);
-          out.put({g.indices[start], g.indices[target], DataValue::from_float((double)cost),
-                   DataValue::from_list(std::move(pl))});  // :88-99
-        };
-        if (!std::isfinite(cost)) {  // :322-323
-          put({});
-          return;
-        }
-        if (ties) {
-          if (target == start) return;  // collect() finds no predecessor of the start (:410-421)
-          std::vector<std::vector<uint32_t>> paths;
+      if (keep_ties) {
+        tied.clear();
+        for (uint64_t e = off[si]; e < off[si + 1]; ++e) tied.push_back({rows[2 * e], rows[2 * e + 1]});
+        std::sort(tied.begin(), tied.end());
+      }
+      for (size_t gi = 0; gi < ng; ++gi) {
+        const uint32_t target = goals[gi];
+        const float c = cost[si * ng + gi];
+        if (!std::isfinite(c)) {  // :322-323
+          put(start, target, c, nullptr, 0);
+        } else if (!keep_ties) {  // :325-333
+          const uint64_t b = off[si * ng + gi];
+          put(start, target, c, rows.data() + b, off[si * ng + gi + 1] - b);
+        } else if (target != start) {  // collect() finds no predecessor of the start (:410-421)
+          paths.clear();
           std::vector<uint32_t> chain{target};
-          collect(g, in_edges, d, start, chain, paths, poison);
-          for (auto& path : paths) put(path);
-        } else {
-          std::vector<uint32_t> path;  // :325-333
-          uint32_t cur = target;
-          while (cur != start) {
-            path.push_back(cur);
-            cur = p[cur];
-          }
-          path.push_back(start);
-          std::reverse(path.begin(), path.end());
-          put(path);
+          collect(tied, start, chain, paths, poison);
+          for (auto& path : paths) put(start, target, c, path.data(), path.size());
         }
-      };
-      if (has_term) {
-        for (uint32_t t : termination_nodes) emit(t);
-      } else {
-        for (uint32_t t = 0; t < n; ++t) emit(t);  // Goal for (): 0..total, :233-235
       }
       poison.check();
     }

@@ -359,6 +359,25 @@ int cozo_gpu_pagerank(cozo_gpu_graph_t* g, float damping, double tol, uint32_t m
 int cozo_gpu_sssp_multi(cozo_gpu_graph_t* g, const uint32_t* sources, uint32_t n_src, float* out_dist,
                         uint32_t* out_pred, double* out_kernel_ms, const volatile int* poison);
 
+/* ShortestPathDijkstra with a termination relation (shortest_path_dijkstra.rs:70-150, 274-339): for every source,
+ * the shortest paths to `goals` only; each search stops once every goal's distance is final, and each chunk of
+ * sources is reduced to its goal answers on the device (host memory O(n_src*n_goals + output), never O(n_src*n)).
+ * goals [n_goals] distinct and < n (EINVAL otherwise).  Pair i = si * n_goals + gi.
+ * out_cost [n_src*n_goals] f32, +inf unreachable.
+ * keep_ties == 0: out_path_off [n_src*n_goals + 1] u64, always written: pair i's path is
+ *   out_paths[off[i] .. off[i+1]), start..goal, empty when unreachable.  The paths are complete in out_paths only
+ *   when off[n_src*n_goals] <= paths_cap (nothing is written past paths_cap); otherwise call again with a larger
+ *   buffer.  out_tie_off / out_tie_edges are not used.
+ * keep_ties != 0: no paths.  Instead, per source si, the tied-predecessor edges that lead back from its goals:
+ *   out_tie_off [n_src + 1] u64, always written; out_tie_edges[2*off[si] .. 2*off[si+1]) holds (v, p) pairs, one per
+ *   CSR edge p -> v with fl32(d[p] + w) == d[v], v != source, v a goal with finite cost or the p of such an edge;
+ *   no particular order within a source.  Same capacity convention with ties_cap (in pairs).
+ * poison polled between source chunks. */
+int cozo_gpu_sssp_goals(cozo_gpu_graph_t* g, const uint32_t* sources, uint32_t n_src, const uint32_t* goals,
+                        uint32_t n_goals, int32_t keep_ties, float* out_cost, uint64_t* out_path_off,
+                        uint32_t* out_paths, uint64_t paths_cap, uint64_t* out_tie_off, uint32_t* out_tie_edges,
+                        uint64_t ties_cap, double* out_kernel_ms, const volatile int* poison);
+
 /* Goal-directed batch of dijkstra calls with ForbiddenEdge / ForbiddenNode sets, the form
  * KShortestPathYen uses (fixed_rule/algos/yen.rs:138,168; shortest_path_dijkstra.rs:188-218,274-339):
  * search i runs from sources[i] to goals[i]; its forbidden nodes are forb_nodes[forb_node_ptr[i] ..

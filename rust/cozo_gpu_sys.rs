@@ -118,6 +118,7 @@ extern "C" {
     pub fn cozo_gpu_graph_export(g: *mut CozoGpuGraph, out_ptr: *mut u32, out_idx: *mut u32, out_w: *mut f32, in_ptr: *mut u32, in_idx: *mut u32) -> c_int;
     pub fn cozo_gpu_pagerank(g: *mut CozoGpuGraph, damping: f32, tol: f64, max_iter: u32, out_scores: *mut f32, out_iters: *mut u32, out_err: *mut f64, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
     pub fn cozo_gpu_sssp_multi(g: *mut CozoGpuGraph, sources: *const u32, n_src: u32, out_dist: *mut f32, out_pred: *mut u32, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
+    pub fn cozo_gpu_sssp_goals(g: *mut CozoGpuGraph, sources: *const u32, n_src: u32, goals: *const u32, n_goals: u32, keep_ties: i32, out_cost: *mut f32, out_path_off: *mut u64, out_paths: *mut u32, paths_cap: u64, out_tie_off: *mut u64, out_tie_edges: *mut u32, ties_cap: u64, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
     pub fn cozo_gpu_sssp_paths(g: *mut CozoGpuGraph, sources: *const u32, goals: *const u32, n_src: u32, forb_node_ptr: *const u32, forb_nodes: *const u32, forb_edge_ptr: *const u32, forb_edge_src: *const u32, forb_edge_dst: *const u32, max_len: u32, out_cost: *mut f32, out_len: *mut u32, out_paths: *mut u32, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
     pub fn cozo_gpu_closeness(g: *mut CozoGpuGraph, out: *mut f32, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
     pub fn cozo_gpu_betweenness(g: *mut CozoGpuGraph, out: *mut f32, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;

@@ -265,26 +265,25 @@ impl FixedRule for PageRankGpu {
 
 // ---------------------------------------------------------------------------------------------
 // ShortestPathDijkstra (algos/shortest_path_dijkstra.rs:32-160)
-//   one cozo_gpu_sssp_multi over all starting nodes; keep_ties=false rebuilds the path from `pred`,
-//   keep_ties=true (only honoured with a termination relation, :85-87) enumerates every tied path from
-//   the device DISTANCES: p precedes v on a shortest path iff fl32(dist[p] + w(p,v)) == dist[v], which is
-//   the predecessor set dijkstra_keep_ties accumulates (:372-380) and walks (:397-426).
+//   without a termination relation: one cozo_gpu_sssp_multi over all starting nodes, one row per node,
+//   the path rebuilt from `pred` (keep_ties is only honoured with a termination relation, :85-87).
+//   with one: cozo_gpu_sssp_goals, where each search stops once its goals are settled (:312-315) and only
+//   the goal answers come back: a path per (start, goal), or with keep_ties the tied-predecessor edges
+//   leading back from the goals, walked as dijkstra_keep_ties walks its predecessor lists (:397-426).
 // ---------------------------------------------------------------------------------------------
+/// `tied`: (v, p) pairs of one source, sorted by v
 fn collect_tied_paths(
-    in_edges: &[Vec<(u32, f32)>], dist: &[f32], start: u32, chain: &mut Vec<u32>, paths: &mut Vec<Vec<u32>>,
-    poison: &Poison,
+    tied: &[(u32, u32)], start: u32, chain: &mut Vec<u32>, paths: &mut Vec<Vec<u32>>, poison: &Poison,
 ) -> Result<()> {
-    let last = *chain.last().unwrap() as usize;
-    for &(p, w) in &in_edges[last] {
-        if !dist[p as usize].is_finite() || dist[p as usize] + w != dist[last] {
-            continue;
-        }
+    let last = *chain.last().unwrap();
+    let from = tied.partition_point(|&(v, _)| v < last);
+    for &(_, p) in tied[from..].iter().take_while(|&&(v, _)| v == last) {
         poison.check()?;
         chain.push(p);
         if p == start {
             paths.push(chain.iter().rev().copied().collect());
         } else {
-            collect_tied_paths(in_edges, dist, start, chain, paths, poison)?;
+            collect_tied_paths(tied, start, chain, paths, poison)?;
         }
         chain.pop();
     }
@@ -314,66 +313,95 @@ impl FixedRule for ShortestPathDijkstraGpu {
         let sources: Vec<u32> = starting_nodes.iter().copied().collect();
         let g = &el.g;
         let pm = PoisonMirror::new(poison.clone());
-        let ties = keep_ties && termination_nodes.is_some();
-        let mut in_edges: Vec<Vec<(u32, f32)>> = vec![];
-        if ties {
-            in_edges.resize(n, vec![]);
-            let (src, dst, w) = el.edges()?;
-            for e in 0..src.len() {
-                in_edges[dst[e] as usize].push((src[e], w[e]));
-            }
-        }
-        let mut dist = vec![0f32; sources.len() * n];
-        let mut pred = vec![0u32; sources.len() * n];
         let mut ms = 0f64;
-        pm.guard(unsafe {
-            cozo_gpu_sssp_multi(
-                g.0, sources.as_ptr(), sources.len() as u32,
-                dist.as_mut_ptr(), pred.as_mut_ptr(), &mut ms, pm.ptr(),
-            )
-        })?;
-        for (si, &start) in sources.iter().enumerate() {
-            let (d, p) = (&dist[si * n..(si + 1) * n], &pred[si * n..(si + 1) * n]);
-            // shortest_path_dijkstra.rs:229-262: with goals, one row per goal (unreachable: cost inf,
-            // empty path); without, one row per node, in node order
-            let targets: Box<dyn Iterator<Item = u32>> = match &termination_nodes {
-                Some(tn) => Box::new(tn.iter().copied()),
-                None => Box::new(0..n as u32),
+        let row = |out: &mut RegularTempStore, start: u32, target: u32, cost: f32, path: &[u32]| {
+            out.put(vec![
+                el.indices[start as usize].clone(),
+                el.indices[target as usize].clone(),
+                DataValue::from(cost as f64),
+                DataValue::List(path.iter().map(|&u| el.indices[u as usize].clone()).collect()),
+            ]);
+        };
+        let goals: Vec<u32> = match &termination_nodes {
+            None => {
+                // Goal for (): one row per node, in node order (:233-235)
+                let mut dist = vec![0f32; sources.len() * n];
+                let mut pred = vec![0u32; sources.len() * n];
+                pm.guard(unsafe {
+                    cozo_gpu_sssp_multi(
+                        g.0, sources.as_ptr(), sources.len() as u32,
+                        dist.as_mut_ptr(), pred.as_mut_ptr(), &mut ms, pm.ptr(),
+                    )
+                })?;
+                for (si, &start) in sources.iter().enumerate() {
+                    let (d, p) = (&dist[si * n..(si + 1) * n], &pred[si * n..(si + 1) * n]);
+                    for target in 0..n as u32 {
+                        let mut path = vec![];
+                        if d[target as usize].is_finite() {
+                            let mut cur = target;
+                            path.push(cur);
+                            while cur != start {
+                                cur = p[cur as usize];
+                                path.push(cur);
+                            }
+                            path.reverse();
+                        }
+                        row(out, start, target, d[target as usize], &path);
+                    }
+                }
+                return Ok(());
+            }
+            Some(tn) => tn.iter().copied().collect(),
+        };
+        // an empty termination set is already exhausted (Goal for BTreeSet, :260-272): no rows
+        if goals.is_empty() {
+            return Ok(());
+        }
+        let (ns, ng) = (sources.len(), goals.len());
+        let mut cost = vec![0f32; ns * ng];
+        let mut off = vec![0u64; if keep_ties { ns + 1 } else { ns * ng + 1 }];
+        let mut rows: Vec<u32>;
+        let mut cap = 16 * (ns * ng) as u64; // a first guess; the call reports the total when it does not fit
+        loop {
+            rows = vec![0u32; (cap.max(1) as usize) * if keep_ties { 2 } else { 1 }];
+            let (po, pp, pc, to, te, tc) = if keep_ties {
+                (ptr::null_mut(), ptr::null_mut(), 0, off.as_mut_ptr(), rows.as_mut_ptr(), cap)
+            } else {
+                (off.as_mut_ptr(), rows.as_mut_ptr(), cap, ptr::null_mut(), ptr::null_mut(), 0)
             };
-            for target in targets {
-                let cost = d[target as usize];
-                if ties && cost.is_finite() {
-                    if target == start {
-                        continue; // no predecessor of the start: the reference emits nothing (:410-421)
-                    }
+            pm.guard(unsafe {
+                cozo_gpu_sssp_goals(
+                    g.0, sources.as_ptr(), ns as u32, goals.as_ptr(), ng as u32, keep_ties as i32,
+                    cost.as_mut_ptr(), po, pp, pc, to, te, tc, &mut ms, pm.ptr(),
+                )
+            })?;
+            let total = *off.last().unwrap();
+            if total <= cap {
+                break;
+            }
+            cap = total;
+        }
+        for (si, &start) in sources.iter().enumerate() {
+            let mut tied: Vec<(u32, u32)> = vec![];
+            if keep_ties {
+                tied = (off[si]..off[si + 1]).map(|e| (rows[2 * e as usize], rows[2 * e as usize + 1])).collect();
+                tied.sort_unstable();
+            }
+            for (gi, &target) in goals.iter().enumerate() {
+                let c = cost[si * ng + gi];
+                if !c.is_finite() {
+                    row(out, start, target, c, &[]); // :322-323
+                } else if !keep_ties {
+                    let (b, e) = (off[si * ng + gi] as usize, off[si * ng + gi + 1] as usize);
+                    row(out, start, target, c, &rows[b..e]); // :325-333
+                } else if target != start {
+                    // no predecessor of the start: the reference emits nothing for it (:410-421)
                     let (mut chain, mut paths) = (vec![target], vec![]);
-                    collect_tied_paths(&in_edges, d, start, &mut chain, &mut paths, &poison)?;
+                    collect_tied_paths(&tied, start, &mut chain, &mut paths, &poison)?;
                     for path in paths {
-                        out.put(vec![
-                            el.indices[start as usize].clone(),
-                            el.indices[target as usize].clone(),
-                            DataValue::from(cost as f64),
-                            DataValue::List(path.into_iter().map(|u| el.indices[u as usize].clone()).collect()),
-                        ]);
+                        row(out, start, target, c, &path);
                     }
-                    continue;
                 }
-                let mut path = vec![];
-                if cost.is_finite() {
-                    let mut cur = target;
-                    path.push(cur);
-                    while cur != start {
-                        cur = p[cur as usize];
-                        path.push(cur);
-                    }
-                    path.reverse();
-                }
-                out.put(vec![
-                    el.indices[start as usize].clone(),
-                    el.indices[target as usize].clone(),
-                    DataValue::from(cost as f64),
-                    DataValue::List(path.into_iter().map(|u| el.indices[u as usize].clone()).collect()),
-                ]);
             }
         }
         Ok(())
