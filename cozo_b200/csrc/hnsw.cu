@@ -4,6 +4,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <type_traits>
 
 #include "hnsw_host.hpp"
 
@@ -41,13 +42,11 @@ struct SearchParams {
 };
 
 
-// hnsw_knn's tail (hnsw.rs:943-956, 997-1006) for the query of this warp: walk the beam nearest first, drop
-// `dist > radius` and rows the filter rejects, keep the first k, pad the rest.  Without a filter the beam is cut to k
-// before the radius test, and without either the kept entries are a prefix of the sorted array.  A radius does not
-// keep a prefix: NaN keys sort last and pass it (`NaN > r` is false).  Returns the number of results.
+// hnsw_knn's tail for the query of this warp (emit_results): into out_ids/out_dist when given, and into every
+// destination's gather buffer.  Returns the number of results.
 __device__ __forceinline__ uint32_t emit_results(const SearchParams& p, const WarpCtx& w, uint32_t qi, int lane,
                                                  bool searched) {
-  auto store = [&](uint32_t i, uint32_t oid, float od) {
+  return emit_results(p, w, w.fd, lane, searched, [&](uint32_t i, uint32_t oid, float od) {
     if (p.out_ids) {
       p.out_ids[(size_t)qi * p.k + i] = oid;
       p.out_dist[(size_t)qi * p.k + i] = od;
@@ -57,32 +56,7 @@ __device__ __forceinline__ uint32_t emit_results(const SearchParams& p, const Wa
       p.dest_ids[d][at] = oid;
       p.dest_dist[d][at] = od;
     }
-  };
-  uint32_t found = 0;
-  if (searched && !p.filter_mask && !p.has_radius) {
-    found = w.len < p.k ? w.len : p.k;
-    for (uint32_t i = lane; i < found; i += 32) store(i, w.fi[i] & IDMASK, w.fd[i]);
-  } else if (searched) {
-    const uint32_t lim = p.filter_mask || w.len < p.k ? w.len : p.k;
-    for (uint32_t base_i = 0; base_i < lim && found < p.k; base_i += 32) {
-      const uint32_t i = base_i + lane;
-      bool ok = i < lim;
-      uint32_t id = 0;
-      float d = 0.f;
-      if (ok) {
-        id = w.fi[i] & IDMASK;
-        d = w.fd[i];
-        ok = (!p.filter_mask || ((p.filter_mask[id >> 5] >> (id & 31)) & 1u)) && !(p.has_radius && (double)d > p.radius);
-      }
-      const uint32_t bal = __ballot_sync(0xffffffffu, ok);
-      const uint32_t pos = found + __popc(bal & ((1u << lane) - 1));
-      if (ok && pos < p.k) store(pos, id, d);
-      found += __popc(bal);
-    }
-    if (found > p.k) found = p.k;
-  }
-  for (uint32_t i = found + lane; i < p.k; i += 32) store(i, NONE, INFINITY);
-  return found;
+  });
 }
 
 #ifdef COZO_HOP_CLOCKS
@@ -944,11 +918,10 @@ extern "C" int cozo_gpu_hnsw_search_scatter_dev(cozo_gpu_hnsw_t* h, const float*
                          nullptr);
 }
 
-static int search_host_impl(cozo_gpu_hnsw_t* h, const float* queries, uint32_t B, uint32_t k, uint32_t ef, double radius,
-                            const uint32_t* row_mask, uint32_t* out_ids, float* out_dist, uint32_t* out_count,
-                            CozoGpuSearchStats* stats) {
-  int rc = check_search_args(h, k, ef);
-  if (rc) return rc;
+template <typename T>
+int cozo::hnsw_search_host(cozo_gpu_hnsw_t* h, const T* queries, uint32_t B, uint32_t k, uint32_t ef, double radius,
+                           const uint32_t* row_mask, uint32_t* out_ids, T* out_dist, uint32_t* out_count,
+                           CozoGpuSearchStats* stats) {
   if (B && (!queries || !out_ids || !out_dist)) return set_error(COZO_GPU_EINVAL, "null buffer");
   if (stats) memset(stats, 0, sizeof(*stats));
   if (B == 0) return 0;
@@ -965,28 +938,31 @@ static int search_host_impl(cozo_gpu_hnsw_t* h, const float* queries, uint32_t B
       return done(set_error(_e == cudaErrorMemoryAllocation ? COZO_GPU_ENOMEM : COZO_GPU_ECUDA,    \
                             "%s failed: %s", #call, cudaGetErrorString(_e)));                     \
   } while (0)
-  const uint32_t dim = h->dev.dim;
-  size_t qf = (size_t)B * dim;
-  if (ws->q_floats < qf) {
+  const size_t qb = (size_t)B * h->dev.dim * sizeof(T), db = (size_t)B * k * sizeof(T);
+  if (ws->q_bytes < qb) {
     if (ws->q) cudaFree(ws->q);
     ws->q = nullptr;
-    ws->q_floats = 0;
-    S_CUDA(cudaMalloc(&ws->q, qf * 4));
-    ws->q_floats = qf;
+    ws->q_bytes = 0;
+    S_CUDA(cudaMalloc(&ws->q, qb));
+    ws->q_bytes = qb;
+  }
+  if (ws->dist_bytes < db) {
+    if (ws->dist) cudaFree(ws->dist);
+    ws->dist = nullptr;
+    ws->dist_bytes = 0;
+    S_CUDA(cudaMalloc(&ws->dist, db));
+    ws->dist_bytes = db;
   }
   if (ws->out_rows < B || ws->out_k < k) {
     if (ws->ids) cudaFree(ws->ids);
-    if (ws->dist) cudaFree(ws->dist);
     if (ws->count) cudaFree(ws->count);
     if (ws->qstats) cudaFree(ws->qstats);
     ws->ids = nullptr;
-    ws->dist = nullptr;
     ws->count = nullptr;
     ws->qstats = nullptr;
     ws->out_rows = ws->out_k = 0;
     size_t rows = std::max<size_t>(B, ws->out_rows), kk = std::max<size_t>(k, ws->out_k);
     S_CUDA(cudaMalloc(&ws->ids, rows * kk * 4));
-    S_CUDA(cudaMalloc(&ws->dist, rows * kk * 4));
     S_CUDA(cudaMalloc(&ws->count, rows * 4));
     S_CUDA(cudaMalloc(&ws->qstats, rows * 16));
     ws->out_rows = rows;
@@ -1004,14 +980,20 @@ static int search_host_impl(cozo_gpu_hnsw_t* h, const float* queries, uint32_t B
     }
     S_CUDA(cudaMemcpyAsync(ws->mask, row_mask, words * 4, cudaMemcpyHostToDevice, st));
   }
-  S_CUDA(cudaMemcpyAsync(ws->q, queries, qf * 4, cudaMemcpyHostToDevice, st));
+  S_CUDA(cudaMemcpyAsync(ws->q, queries, qb, cudaMemcpyHostToDevice, st));
   S_CUDA(cudaEventRecord(ws->e0, st));
-  rc = hnsw_launch_search(h, ws, ws->q, B, k, ef, radius, ws->ids, ws->dist, ws->count, ws->qstats, st, nullptr,
-                          row_mask ? ws->mask : nullptr);
+  const uint32_t* mask = row_mask ? ws->mask : nullptr;
+  int rc;
+  if constexpr (std::is_same_v<T, double>)
+    rc = hnsw_launch_search_f64(h, ws, static_cast<const double*>(ws->q), B, k, ef, radius, ws->ids,
+                                static_cast<double*>(ws->dist), ws->count, ws->qstats, st, nullptr, mask);
+  else
+    rc = hnsw_launch_search(h, ws, static_cast<const float*>(ws->q), B, k, ef, radius, ws->ids,
+                            static_cast<float*>(ws->dist), ws->count, ws->qstats, st, nullptr, mask);
   if (rc) return done(rc);
   S_CUDA(cudaEventRecord(ws->e1, st));
   S_CUDA(cudaMemcpyAsync(out_ids, ws->ids, (size_t)B * k * 4, cudaMemcpyDeviceToHost, st));
-  S_CUDA(cudaMemcpyAsync(out_dist, ws->dist, (size_t)B * k * 4, cudaMemcpyDeviceToHost, st));
+  S_CUDA(cudaMemcpyAsync(out_dist, ws->dist, db, cudaMemcpyDeviceToHost, st));
   if (out_count) S_CUDA(cudaMemcpyAsync(out_count, ws->count, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
   std::vector<uint32_t> qs;
   if (stats) {
@@ -1033,18 +1015,24 @@ static int search_host_impl(cozo_gpu_hnsw_t* h, const float* queries, uint32_t B
 #undef S_CUDA
   return done(0);
 }
+template int cozo::hnsw_search_host<double>(cozo_gpu_hnsw_t*, const double*, uint32_t, uint32_t, uint32_t, double,
+                                            const uint32_t*, uint32_t*, double*, uint32_t*, CozoGpuSearchStats*);
 
 extern "C" int cozo_gpu_hnsw_search(cozo_gpu_hnsw_t* h, const float* queries, uint32_t B, uint32_t k, uint32_t ef,
                                     double radius, uint32_t* out_ids, float* out_dist, uint32_t* out_count,
                                     CozoGpuSearchStats* stats) {
-  return search_host_impl(h, queries, B, k, ef, radius, nullptr, out_ids, out_dist, out_count, stats);
+  int rc = check_search_args(h, k, ef);
+  if (rc) return rc;
+  return hnsw_search_host(h, queries, B, k, ef, radius, nullptr, out_ids, out_dist, out_count, stats);
 }
 
 extern "C" int cozo_gpu_hnsw_search_filtered(cozo_gpu_hnsw_t* h, const float* queries, uint32_t B, uint32_t k,
                                              uint32_t ef, double radius, const uint32_t* row_mask, uint32_t* out_ids,
                                              float* out_dist, uint32_t* out_count, CozoGpuSearchStats* stats) {
   if (h && h->dev.n && !row_mask) return set_error(COZO_GPU_EINVAL, "null row mask");
-  return search_host_impl(h, queries, B, k, ef, radius, row_mask, out_ids, out_dist, out_count, stats);
+  int rc = check_search_args(h, k, ef);
+  if (rc) return rc;
+  return hnsw_search_host(h, queries, B, k, ef, radius, row_mask, out_ids, out_dist, out_count, stats);
 }
 
 extern "C" int cozo_gpu_hnsw_search_filtered_dev(cozo_gpu_hnsw_t* h, const float* queries_dev, uint32_t B, uint32_t k,

@@ -289,14 +289,16 @@ __device__ __forceinline__ float dist_ldg1(const float4 (&q)[NV], const float4* 
   return finish<METRIC>(a0, b0, qnorm);
 }
 
-// found_nn.push + pop-if-over-ef (hnsw.rs:577-580) on the sorted array.
-// Precondition: len < ef || d < fd[len-1].  Equal keys keep arrival order.  Keys are ordered as OrderedFloat orders
-// them: NaN after every number (+inf included) and equal to NaN, so a NaN key goes behind every other key.
-__device__ __forceinline__ void sorted_insert(WarpCtx& w, uint32_t ef, float d, uint32_t id, int lane) {
+// found_nn.push + pop-if-over-ef (hnsw.rs:577-580) on the sorted array: keys fd (w.fd in the f32 searches, f64 keys in
+// the F64 one), ids w.fi.  Precondition: len < ef || d < fd[len-1].  Equal keys keep arrival order.  Keys are ordered
+// as OrderedFloat orders them: NaN after every number (+inf included) and equal to NaN, so a NaN key goes behind every
+// other key.
+template <typename K>
+__device__ __forceinline__ void sorted_insert(WarpCtx& w, K* fd, uint32_t ef, K d, uint32_t id, int lane) {
   uint32_t pos = 0;
   for (uint32_t base = 0; base < w.len; base += 32) {
     uint32_t i = base + lane;
-    bool le = (i < w.len) && (w.fd[i] <= d || d != d);
+    bool le = (i < w.len) && (fd[i] <= d || d != d);
     uint32_t bal = __ballot_sync(0xffffffffu, le);
     pos += __popc(bal);
     if (bal != 0xffffffffu) break;
@@ -305,27 +307,34 @@ __device__ __forceinline__ void sorted_insert(WarpCtx& w, uint32_t ef, float d, 
   for (int top = (int)newlen - 1; top > (int)pos; top -= 32) {
     int i = top - 1 - lane;
     bool act = i >= (int)pos;
-    float td = 0.f;
+    K td = 0;
     uint32_t ti = 0;
     if (act) {
-      td = w.fd[i];
+      td = fd[i];
       ti = w.fi[i];
     }
     __syncwarp();
     if (act) {
-      w.fd[i + 1] = td;
+      fd[i + 1] = td;
       w.fi[i + 1] = ti;
     }
     __syncwarp();
   }
   __syncwarp();  // every lane has finished reading fd[len-1] / the shifted slots (vote ops do not order memory)
   if (lane == 0) {
-    w.fd[pos] = d;
+    fd[pos] = d;
     w.fi[pos] = id;
   }
   __syncwarp();
   w.len = newlen;
   if (pos < w.cursor) w.cursor = pos;
+}
+
+// the admission of one evaluated neighbour (hnsw.rs:575-581).  d by reference: compared as a value the key is an
+// argument, which the compiler's canonical form orders after the load of fd[len-1], flipping the test in the callers.
+template <typename K>
+__device__ __forceinline__ void admit(WarpCtx& w, K* fd, uint32_t ef, const K& d, uint32_t id, int lane) {
+  if (w.len < ef || d < fd[w.len - 1]) sorted_insert(w, fd, ef, d, id, lane);
 }
 
 // visited.insert for the ids in `id` (one per lane, NONE = idle); returns whether
@@ -344,6 +353,101 @@ __device__ __forceinline__ bool visit_mark(WarpCtx& w, uint32_t id, int lane, ui
   }
   w.nlog += __popc(newmask);
   return isnew;
+}
+
+// visited <- keys(found); candidates <- found (hnsw.rs:554-557)
+__device__ __forceinline__ void seed_visited(WarpCtx& w, int lane) {
+  for (uint32_t base = 0; base < w.len; base += 32) {
+    uint32_t i = base + lane;
+    uint32_t id = NONE;
+    if (i < w.len) {
+      id = w.fi[i] & IDMASK;
+      w.fi[i] = id;
+    }
+    uint32_t nm;
+    visit_mark(w, id, lane, nm);
+  }
+  __syncwarp();
+  w.cursor = 0;
+}
+
+// candidates.pop() (hnsw.rs:559): the nearest not-yet-expanded entry into `cand`, marked expanded.  false when there is
+// none, which is the reference's `candidate_dist > furthest_dist` break (hnsw.rs:562).  (A flag rather than a NONE id:
+// the compiler cannot tell that a popped id is never NONE, and would keep that test in every search loop.)
+__device__ __forceinline__ bool pop_candidate(const HnswDev& g, WarpCtx& w, uint32_t level, int lane, uint32_t& cand) {
+  uint32_t ci = NONE;
+  for (uint32_t base = w.cursor & ~31u; base < w.len; base += 32) {
+    uint32_t i = base + lane;
+    bool un = (i < w.len) && (i >= w.cursor) && !(w.fi[i] & EXPANDED);
+    uint32_t bal = __ballot_sync(0xffffffffu, un);
+    if (bal) {
+      ci = base + __ffs(bal) - 1;
+      break;
+    }
+  }
+  if (ci == NONE) return false;
+  cand = w.fi[ci];
+  __syncwarp();
+  if (lane == 0) w.fi[ci] = cand | EXPANDED;
+  w.cursor = ci + 1;
+  w.nodes_expanded++;
+  if (level == 0 && ci + 1 + lane < w.len && lane < 2) {
+    // the next pop is most likely one of the following entries: pull their adjacency rows into L2
+    uint32_t nxt = w.fi[ci + 1 + lane];
+    if (!(nxt & EXPANDED)) prefetch_l2(g.adj0 + (size_t)nxt * g.s0);
+  }
+  return true;
+}
+
+// hnsw_get_neighbours (hnsw.rs:588-629): the padded adjacency row of `cand` on `level`
+__device__ __forceinline__ const uint32_t* neighbour_row(const HnswDev& g, uint32_t cand, uint32_t level) {
+  return level == 0 ? g.adj0 + (size_t)cand * g.s0 : g.adj_up + (size_t)(g.upper_off[cand] + level - 1) * g.su;
+}
+
+// the unvisited ids of one adjacency chunk (hnsw.rs:569-571,582): marks them visited, compacts them into pend in
+// neighbour order, counts them as evaluations and returns how many there are
+__device__ __forceinline__ uint32_t take_unvisited(WarpCtx& w, uint32_t id, int lane, uint32_t* pend) {
+  uint32_t newmask;
+  const bool isnew = visit_mark(w, id, lane, newmask);
+  const uint32_t cnt = __popc(newmask);
+  if (isnew) pend[__popc(newmask & ((1u << lane) - 1))] = id;
+  w.dist_evals += cnt;
+  return cnt;
+}
+
+// hnsw_knn's tail (hnsw.rs:943-956, 997-1006) for the query of this warp: walk the beam (keys fd) nearest first, drop
+// `dist > radius` and rows the filter rejects, keep the first k, pad the rest with (NONE, +inf).  Without a filter the
+// beam is cut to k before the radius test, and without either the kept entries are a prefix of the sorted array.  A
+// radius does not keep a prefix: NaN keys sort last and pass it (`NaN > r` is false).  p supplies k, has_radius, radius
+// and filter_mask (SearchParams, Search64Params); store(i, id, dist) writes result i.  Returns the number of results.
+template <typename K, typename P, typename Store>
+__device__ __forceinline__ uint32_t emit_results(const P& p, const WarpCtx& w, const K* fd, int lane, bool searched,
+                                                 const Store& store) {
+  uint32_t found = 0;
+  if (searched && !p.filter_mask && !p.has_radius) {
+    found = w.len < p.k ? w.len : p.k;
+    for (uint32_t i = lane; i < found; i += 32) store(i, w.fi[i] & IDMASK, fd[i]);
+  } else if (searched) {
+    const uint32_t lim = p.filter_mask || w.len < p.k ? w.len : p.k;
+    for (uint32_t base_i = 0; base_i < lim && found < p.k; base_i += 32) {
+      const uint32_t i = base_i + lane;
+      bool ok = i < lim;
+      uint32_t id = 0;
+      K d = 0;
+      if (ok) {
+        id = w.fi[i] & IDMASK;
+        d = fd[i];
+        ok = (!p.filter_mask || ((p.filter_mask[id >> 5] >> (id & 31)) & 1u)) && !(p.has_radius && (double)d > p.radius);
+      }
+      const uint32_t bal = __ballot_sync(0xffffffffu, ok);
+      const uint32_t pos = found + __popc(bal & ((1u << lane) - 1));
+      if (ok && pos < p.k) store(pos, id, d);
+      found += __popc(bal);
+    }
+    if (found > p.k) found = p.k;
+  }
+  for (uint32_t i = found + lane; i < p.k; i += 32) store(i, NONE, (K)INFINITY);
+  return found;
 }
 
 // Clearing by the log costs one random atomic per logged id; by the sweep, one coalesced 16-byte store per 4 words.  A
@@ -571,7 +675,7 @@ __device__ __forceinline__ void prune_chunk(const HnswDev& g, WarpCtx& w, const 
     fin &= fin - 1;
     __syncwarp();
     if (d < w.fd[ef - 1]) {  // hnsw.rs:575-581 (the beam stays full)
-      sorted_insert(w, ef, d, nid, lane);
+      sorted_insert(w, w.fd, ef, d, nid, lane);
       WE = radius(w.fd[ef - 1]);
     }
     HOP_ADD(w, HC_FSCORE, t2);
@@ -648,54 +752,14 @@ __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const
                                              const QueryCodes* qc = nullptr) {
   const int nvec4 = g.ld >> 2;
   const uint32_t row_bytes = g.ld * 4;
-  // visited <- keys(found); candidates <- found (hnsw.rs:554-557)
-  for (uint32_t base = 0; base < w.len; base += 32) {
-    uint32_t i = base + lane;
-    uint32_t id = NONE;
-    if (i < w.len) {
-      id = w.fi[i] & IDMASK;
-      w.fi[i] = id;
-    }
-    uint32_t nm;
-    visit_mark(w, id, lane, nm);
-  }
-  __syncwarp();
-  w.cursor = 0;
+  seed_visited(w, lane);
   const uint32_t stride = level == 0 ? g.s0 : g.su;
 
   for (;;) {
     HOP_T(tp);
-    // candidates.pop(): nearest not-yet-expanded entry (hnsw.rs:559)
-    uint32_t ci = NONE;
-    for (uint32_t base = w.cursor & ~31u; base < w.len; base += 32) {
-      uint32_t i = base + lane;
-      bool un = (i < w.len) && (i >= w.cursor) && !(w.fi[i] & EXPANDED);
-      uint32_t bal = __ballot_sync(0xffffffffu, un);
-      if (bal) {
-        ci = base + __ffs(bal) - 1;
-        break;
-      }
-    }
-    if (ci == NONE) break;  // == `candidate_dist > furthest_dist` break (hnsw.rs:562)
-    uint32_t cand = w.fi[ci];
-    __syncwarp();
-    if (lane == 0) w.fi[ci] = cand | EXPANDED;
-    w.cursor = ci + 1;
-    w.nodes_expanded++;
-    if (level == 0 && ci + 1 + lane < w.len && lane < 2) {
-      // the next pop is most likely one of the following entries: pull their adjacency rows into L2
-      uint32_t nxt = w.fi[ci + 1 + lane];
-      if (!(nxt & EXPANDED))
-        prefetch_l2(g.adj0 + (size_t)nxt * g.s0);
-    }
-    // hnsw_get_neighbours (hnsw.rs:588-629): one padded row
-    const uint32_t* row;
-    if (level == 0) {
-      row = g.adj0 + (size_t)cand * g.s0;
-    } else {
-      uint32_t off = g.upper_off[cand];
-      row = g.adj_up + (size_t)(off + level - 1) * g.su;
-    }
+    uint32_t cand;
+    if (!pop_candidate(g, w, level, lane, cand)) break;
+    const uint32_t* row = neighbour_row(g, cand, level);
     for (uint32_t nb = 0; nb < stride; nb += 32) {
       if (nb) HOP_SET(tp);
       uint32_t id = __ldg(row + nb + lane);
@@ -711,13 +775,9 @@ __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const
         }
       }
       HOP_T(tv);
-      uint32_t newmask;
-      bool isnew = visit_mark(w, id, lane, newmask);  // hnsw.rs:569-571,582
-      uint32_t cnt = __popc(newmask);
-      if (isnew) w.pend[__popc(newmask & ((1u << lane) - 1))] = id;
+      const uint32_t cnt = take_unvisited(w, id, lane, w.pend);
       __syncwarp();
       HOP_ADD(w, HC_VISIT, tv);
-      w.dist_evals += cnt;
       if (BULK) {
         // ring indices advance by compare-and-wrap (a runtime `% ns` costs ~20 instructions)
         uint32_t issued = 0, si = w.head, sc = w.head;
@@ -741,7 +801,7 @@ __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const
           if (++sc == w.ns) sc = 0;
           uint32_t nid = w.pend[c];
           __syncwarp();
-          if (w.len < ef || d < w.fd[w.len - 1]) sorted_insert(w, ef, d, nid, lane);  // hnsw.rs:575-581
+          admit(w, w.fd, ef, d, nid, lane);
           HOP_ADD(w, HC_FSCORE, ts);
         }
         w.head = sc;
@@ -760,8 +820,8 @@ __device__ __forceinline__ void search_level(const HnswDev& g, WarpCtx& w, const
                                        qnorm);
             d1 = 0.f;
           }
-          if (w.len < ef || d0 < w.fd[w.len - 1]) sorted_insert(w, ef, d0, id0, lane);
-          if (two && (w.len < ef || d1 < w.fd[w.len - 1])) sorted_insert(w, ef, d1, id1, lane);
+          admit(w, w.fd, ef, d0, id0, lane);
+          if (two) admit(w, w.fd, ef, d1, id1, lane);
         }
       }
       __syncwarp();
@@ -795,50 +855,18 @@ __device__ __forceinline__ void coop_search_level(const HnswDev& g, WarpCtx& w, 
   // warp-0 state of the current expansion
   const uint32_t* row = nullptr;
   uint32_t nb = stride;  // chunk offset inside the candidate's adjacency row; stride = need a new candidate
-  if (warp == 0) {
-    for (uint32_t base = 0; base < w.len; base += 32) {  // visited <- keys(found) (hnsw.rs:554-557)
-      uint32_t i = base + lane;
-      uint32_t id = NONE;
-      if (i < w.len) {
-        id = w.fi[i] & IDMASK;
-        w.fi[i] = id;
-      }
-      uint32_t nm;
-      visit_mark(w, id, lane, nm);
-    }
-    __syncwarp();
-    w.cursor = 0;
-  }
+  if (warp == 0) seed_visited(w, lane);
   for (;;) {
     if (warp == 0) {
       uint32_t cnt = 0;
       while (cnt == 0) {
-        if (nb >= stride) {  // candidates.pop() (hnsw.rs:559)
-          uint32_t ci = NONE;
-          for (uint32_t base = w.cursor & ~31u; base < w.len; base += 32) {
-            uint32_t i = base + lane;
-            bool un = (i < w.len) && (i >= w.cursor) && !(w.fi[i] & EXPANDED);
-            uint32_t bal = __ballot_sync(0xffffffffu, un);
-            if (bal) {
-              ci = base + __ffs(bal) - 1;
-              break;
-            }
-          }
-          if (ci == NONE) {
+        if (nb >= stride) {
+          uint32_t cand;
+          if (!pop_candidate(g, w, level, lane, cand)) {
             cnt = COOP_DONE;
             break;
           }
-          uint32_t cand = w.fi[ci];
-          __syncwarp();
-          if (lane == 0) w.fi[ci] = cand | EXPANDED;
-          w.cursor = ci + 1;
-          w.nodes_expanded++;
-          if (level == 0 && ci + 1 + lane < w.len && lane < 2) {
-            uint32_t nxt = w.fi[ci + 1 + lane];
-            if (!(nxt & EXPANDED)) prefetch_l2(g.adj0 + (size_t)nxt * g.s0);
-          }
-          row = level == 0 ? g.adj0 + (size_t)cand * g.s0
-                           : g.adj_up + (size_t)(g.upper_off[cand] + level - 1) * g.su;
+          row = neighbour_row(g, cand, level);
           nb = 0;
         }
         uint32_t id = __ldg(row + nb + lane);
@@ -846,11 +874,7 @@ __device__ __forceinline__ void coop_search_level(const HnswDev& g, WarpCtx& w, 
         nb = validmask ? nb + 32 : stride;  // rows are packed: an empty chunk ends the row
         if (!validmask) continue;
         w.nbr_reads += __popc(validmask);
-        uint32_t newmask;
-        bool isnew = visit_mark(w, id, lane, newmask);
-        cnt = __popc(newmask);
-        if (isnew) cs.pend[__popc(newmask & ((1u << lane) - 1))] = id;
-        w.dist_evals += cnt;
+        cnt = take_unvisited(w, id, lane, cs.pend);
       }
       if (lane == 0) cs.ctrl[0] = cnt;
     }
@@ -885,7 +909,7 @@ __device__ __forceinline__ void coop_search_level(const HnswDev& g, WarpCtx& w, 
         const float d = cs.pdist[c];
         const uint32_t nid = cs.pend[c];
         __syncwarp();
-        if (w.len < ef || d < w.fd[w.len - 1]) sorted_insert(w, ef, d, nid, lane);
+        admit(w, w.fd, ef, d, nid, lane);
       }
     }
   }

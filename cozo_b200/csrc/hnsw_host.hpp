@@ -15,11 +15,12 @@ struct HnswWorkspace {
   uint32_t* vlog = nullptr;
   size_t vlog_words = 0;
   uint32_t* counter = nullptr;
-  // staging buffers of the host-pointer API
-  float* q = nullptr;
-  size_t q_floats = 0;
+  // staging buffers of the host-pointer API (q and dist hold f32 or f64 elements)
+  void* q = nullptr;
+  size_t q_bytes = 0;
+  void* dist = nullptr;
+  size_t dist_bytes = 0;
   uint32_t* ids = nullptr;
-  float* dist = nullptr;
   uint32_t* count = nullptr;
   uint32_t* qstats = nullptr;
   size_t out_rows = 0, out_k = 0;
@@ -136,6 +137,13 @@ int hnsw_launch_search_f64(cozo_gpu_hnsw* h, HnswWorkspace* ws, const double* d_
 // merge.cu: cozo_gpu_topk_merge_dev on F64 distances
 int topk_merge_f64_dev(const double* dist_dev, const uint32_t* ids_dev, uint32_t n_shards, uint32_t B, uint32_t k,
                        const uint64_t* shard_offsets_dev, uint64_t* out_ids_dev, double* out_dist_dev, void* stream);
+// the host-pointer search of cozo_gpu_hnsw_search / _filtered (T = float) and cozo_gpu_hnsw_search_f64 (T = double),
+// after the entry point's handle, k and ef checks: stages the queries and the row mask through a workspace, runs the
+// search and copies the results and the summed counters back
+template <typename T>
+int hnsw_search_host(cozo_gpu_hnsw* h, const T* queries, uint32_t B, uint32_t k, uint32_t ef, double radius,
+                     const uint32_t* row_mask, uint32_t* out_ids, T* out_dist, uint32_t* out_count,
+                     CozoGpuSearchStats* stats);
 HnswWorkspace* hnsw_acquire_ws(cozo_gpu_hnsw* h);
 void hnsw_release_ws(cozo_gpu_hnsw* h, HnswWorkspace* ws);
 int hnsw_ws_reserve(HnswWorkspace* ws, size_t vis_words, size_t vlog_words, cudaStream_t stream);
