@@ -32,7 +32,8 @@ EXPORTS = [
     "cozo_gpu_hnsw_search_filtered", "cozo_gpu_hnsw_search_filtered_dev", "cozo_gpu_hnsw_search_f64",
     "cozo_gpu_graph_stage_keys", "cozo_gpu_graph_node_endpoints", "cozo_gpu_graph_lookup_keys",
     "cozo_gpu_hnsw_search_sharded_filtered", "cozo_gpu_hnsw_search_sharded_filtered_dev",
-    "cozo_gpu_hnsw_search_sharded_f64",
+    "cozo_gpu_hnsw_search_sharded_f64", "cozo_gpu_graph_attach_sharded", "cozo_gpu_closeness_sharded",
+    "cozo_gpu_betweenness_sharded", "cozo_gpu_sssp_goals_sharded",
 ]
 UID_BYTES = 128
 
@@ -133,6 +134,10 @@ def load():
     L.cozo_gpu_hnsw_search_sharded_filtered_dev.argtypes = [vp, vp, u32, u32, u32, f64, vp, vp, vp, vp, vp]
     L.cozo_gpu_hnsw_search_sharded_f64.argtypes = [vp, vp, u32, u32, u32, f64, C.c_int, vp, vp, vp, vp,
                                                    C.POINTER(SearchStats)]
+    L.cozo_gpu_graph_attach_sharded.argtypes = [vp, vp]
+    L.cozo_gpu_closeness_sharded.argtypes = [vp, vp, vp, vp]
+    L.cozo_gpu_betweenness_sharded.argtypes = [vp, vp, vp, vp]
+    L.cozo_gpu_sssp_goals_sharded.argtypes = [vp, vp, u32, vp, u32, C.c_int32, vp, vp, vp, u64, vp, vp, u64, vp, vp]
     _lib = L
     return L
 
@@ -398,6 +403,7 @@ class ShardGroup:
         self._h = h
         self.rank, self.world = rank, world
         self.index = None
+        self.graph = None
         self.offset = self.total_rows = 0
 
     @staticmethod
@@ -461,6 +467,30 @@ class ShardGroup:
         else:
             _check(load().cozo_gpu_hnsw_search_sharded_filtered_dev(self._h, q_ptr, B, k, ef, r, row_mask_ptr,
                                                                     out_ids_ptr, out_dist_ptr, qstats_ptr, stream))
+
+    # -- source-sharded graph calls: the same graph staged on every rank, the sources split over the ranks ----------
+    def attach_graph(self, graph: "Graph"):
+        """collective: register this rank's copy of the replicated graph; EINVAL on every rank if the copies differ"""
+        _check(load().cozo_gpu_graph_attach_sharded(self._h, graph._h))
+        self.graph = graph
+
+    def closeness(self, poison=None):
+        """collective cozo_gpu_closeness over the attached graph -> (out f32 [n], this rank's kernel ms)"""
+        out = np.zeros(self.graph.n, np.float32)
+        ms = C.c_double()
+        _check(load().cozo_gpu_closeness_sharded(self._h, _p(out), C.byref(ms), _p(poison)))
+        return out, ms.value
+
+    def betweenness(self, poison=None):
+        """collective cozo_gpu_betweenness over the attached graph -> (out f32 [n], this rank's kernel ms)"""
+        out = np.zeros(self.graph.n, np.float32)
+        ms = C.c_double()
+        _check(load().cozo_gpu_betweenness_sharded(self._h, _p(out), C.byref(ms), _p(poison)))
+        return out, ms.value
+
+    def sssp_goals(self, sources, goals, keep_ties=False, poison=None, cap=None):
+        """collective Graph.sssp_goals over the attached graph, the sources split over the ranks; same results"""
+        return _sssp_goals(load().cozo_gpu_sssp_goals_sharded, self._h, sources, goals, keep_ties, poison, cap)
 
     def close(self):
         if self._h:
@@ -607,27 +637,7 @@ class Graph:
         start..goal ([] when unreachable), as a list of n_src lists; with keep_ties, per source the tied-predecessor
         edges leading back from its goals, a u32 array [k, 2] of (v, p).  The first call has room for `cap` path nodes
         or tie edges (default: 64 per pair) and is repeated with the reported total when that is too small."""
-        sources = np.ascontiguousarray(sources, np.uint32)
-        goals = np.ascontiguousarray(goals, np.uint32)
-        ns, ng = sources.size, goals.size
-        cap = 64 * ns * ng if cap is None else int(cap)
-        while True:
-            cost = np.zeros((ns, ng), np.float32)
-            off = np.zeros((ns + 1) if keep_ties else (ns * ng + 1), np.uint64)
-            rows = np.zeros(max(cap, 1) * (2 if keep_ties else 1), np.uint32)
-            ms = C.c_double()
-            args = (None, None, 0, _p(off), _p(rows), cap) if keep_ties else (_p(off), _p(rows), cap, None, None, 0)
-            _check(load().cozo_gpu_sssp_goals(self._h, _p(sources), ns, _p(goals), ng, int(bool(keep_ties)), _p(cost),
-                                              *args, C.byref(ms), _p(poison)))
-            if int(off[-1]) <= cap:
-                break
-            cap = int(off[-1])
-        off = off.astype(np.int64)
-        if keep_ties:
-            edges = rows[:2 * off[-1]].reshape(-1, 2)
-            return cost, [edges[off[i]:off[i + 1]] for i in range(ns)], ms.value
-        paths = [rows[off[i]:off[i + 1]].tolist() for i in range(ns * ng)]
-        return cost, [paths[i * ng:(i + 1) * ng] for i in range(ns)], ms.value
+        return _sssp_goals(load().cozo_gpu_sssp_goals, self._h, sources, goals, keep_ties, poison, cap)
 
     def clustering(self, poison=None):
         cc = np.zeros(self.n, np.float64)
@@ -647,3 +657,35 @@ class Graph:
             self.close()
         except Exception:
             pass
+
+
+def sssp_goals_once(entry, handle, sources, goals, keep_ties, cap, poison=None):
+    """one raw cozo_gpu_sssp_goals[_sharded] call with room for `cap` rows -> (cost [ns, ng], offsets u64, rows u32,
+    kernel ms); the rows are complete only when offsets[-1] <= cap"""
+    sources = np.ascontiguousarray(sources, np.uint32)
+    goals = np.ascontiguousarray(goals, np.uint32)
+    ns, ng = sources.size, goals.size
+    cost = np.zeros((ns, ng), np.float32)
+    off = np.zeros((ns + 1) if keep_ties else (ns * ng + 1), np.uint64)
+    rows = np.zeros(max(cap, 1) * (2 if keep_ties else 1), np.uint32)
+    ms = C.c_double()
+    args = (None, None, 0, _p(off), _p(rows), cap) if keep_ties else (_p(off), _p(rows), cap, None, None, 0)
+    _check(entry(handle, _p(sources), ns, _p(goals), ng, int(bool(keep_ties)), _p(cost), *args, C.byref(ms),
+                 _p(poison)))
+    return cost, off, rows, ms.value
+
+
+def _sssp_goals(entry, handle, sources, goals, keep_ties, poison, cap):
+    ns, ng = np.size(sources), np.size(goals)
+    cap = 64 * ns * ng if cap is None else int(cap)
+    while True:
+        cost, off, rows, ms = sssp_goals_once(entry, handle, sources, goals, keep_ties, cap, poison)
+        if int(off[-1]) <= cap:
+            break
+        cap = int(off[-1])
+    off = off.astype(np.int64)
+    if keep_ties:
+        edges = rows[:2 * off[-1]].reshape(-1, 2)
+        return cost, [edges[off[i]:off[i + 1]] for i in range(ns)], ms
+    paths = [rows[off[i]:off[i + 1]].tolist() for i in range(ns * ng)]
+    return cost, [paths[i * ng:(i + 1) * ng] for i in range(ns)], ms

@@ -383,38 +383,24 @@ extern "C" int cozo_gpu_sssp_multi(cozo_gpu_graph_t* g, const uint32_t* sources,
   return rc;
 }
 
-extern "C" int cozo_gpu_sssp_goals(cozo_gpu_graph_t* g, const uint32_t* sources, uint32_t n_src, const uint32_t* goals,
-                                   uint32_t n_goals, int32_t keep_ties, float* out_cost, uint64_t* out_path_off,
-                                   uint32_t* out_paths, uint64_t paths_cap, uint64_t* out_tie_off,
-                                   uint32_t* out_tie_edges, uint64_t ties_cap, double* out_kernel_ms,
-                                   const volatile int* poison) {
-  const uint64_t pairs = (uint64_t)n_src * n_goals;
-  uint64_t* off_out = keep_ties ? out_tie_off : out_path_off;
-  uint32_t* rows_out = keep_ties ? out_tie_edges : out_paths;
-  const uint64_t cap = keep_ties ? ties_cap : paths_cap;
-  if (!g || (n_src && !sources) || (n_goals && !goals) || (pairs && !out_cost) || !off_out || (cap && !rows_out))
-    return set_error(COZO_GPU_EINVAL, "null argument");
-  int rc = ensure_init();
-  if (rc) return rc;
-  if (out_kernel_ms) *out_kernel_ms = 0;
+int cozo::sssp_goals_check(cozo_gpu_graph_t* g, const uint32_t* sources, uint32_t n_src, const uint32_t* goals,
+                           uint32_t n_goals) {
   const uint32_t n = g->n;
   for (uint32_t i = 0; i < n_src; ++i)
     if (sources[i] >= n) return set_error(COZO_GPU_EINVAL, "source %u out of range", sources[i]);
-  {
-    std::vector<uint32_t> sorted(goals, goals + n_goals);
-    std::sort(sorted.begin(), sorted.end());
-    for (uint32_t i = 0; i < n_goals; ++i) {
-      if (sorted[i] >= n) return set_error(COZO_GPU_EINVAL, "goal %u out of range", sorted[i]);
-      if (i && sorted[i] == sorted[i - 1]) return set_error(COZO_GPU_EINVAL, "goal %u given twice", sorted[i]);
-    }
+  std::vector<uint32_t> sorted(goals, goals + n_goals);
+  std::sort(sorted.begin(), sorted.end());
+  for (uint32_t i = 0; i < n_goals; ++i) {
+    if (sorted[i] >= n) return set_error(COZO_GPU_EINVAL, "goal %u out of range", sorted[i]);
+    if (i && sorted[i] == sorted[i - 1]) return set_error(COZO_GPU_EINVAL, "goal %u given twice", sorted[i]);
   }
-  // offsets per pair (paths) or per source (tied edges); a source with no goals has none of either
-  const uint64_t n_off = keep_ties ? (uint64_t)n_src + 1 : pairs + 1;
-  std::fill(off_out, off_out + n_off, 0);
-  if (pairs == 0) return 0;
-  CallStream cs;
-  rc = cs.init();
-  if (rc) return rc;
+  return 0;
+}
+
+int cozo::sssp_goals_run(cozo_gpu_graph_t* g, CallStream& cs, const uint32_t* sources, uint32_t n_src,
+                         const uint32_t* goals, uint32_t n_goals, bool keep_ties, float* out_cost, uint64_t* off_out,
+                         uint64_t cap, const volatile int* poison, const GoalRowSink& sink) {
+  const uint32_t n = g->n;
   DevBuf dgoal, dcost, dscan, dmark, drows, tmp;
   COZO_CUDA(cudaMalloc(&dgoal.p, (size_t)n_goals * 4));
   COZO_CUDA(cudaMemcpyAsync(dgoal.p, goals, (size_t)n_goals * 4, cudaMemcpyHostToDevice, cs.s));
@@ -422,7 +408,7 @@ extern "C" int cozo_gpu_sssp_goals(cozo_gpu_graph_t* g, const uint32_t* sources,
   uint64_t base = 0, rows_cap = 0;  // rows so far; capacity of drows in rows (a path node, or one (v, p) pair)
   bool fits = true;
   size_t tmp_bytes = 0;
-  rc = sssp_chunks(
+  return sssp_chunks(
       g, cs, sources, n_src, (size_t)n_goals * 12 + (keep_ties ? (size_t)n + 8 : 0), poison,
       [&](uint32_t s0, uint32_t c, unsigned long long* state, uint32_t* dsrc) -> int {
         const uint64_t pc = (uint64_t)c * n_goals;
@@ -465,17 +451,60 @@ extern "C" int cozo_gpu_sssp_goals(cozo_gpu_graph_t* g, const uint32_t* sources,
             sssp_goal_path_kernel<<<(uint32_t)((pc + 255) / 256), 256, 0, cs.s>>>(state, n, gs.goals, n_goals, c, scan,
                                                                                  drows.as<uint32_t>());
           COZO_CUDA(cudaGetLastError());
-          const uint64_t per_row = keep_ties ? 2 : 1;
-          COZO_CUDA(cudaMemcpyAsync(rows_out + base * per_row, drows.p, total * per_row * 4, cudaMemcpyDeviceToHost,
-                                    cs.s));
+          const int rc = sink(drows.as<uint32_t>(), base, total);
+          if (rc) return rc;
         }
         base += total;
         return 0;
       },
       gs);
+}
+
+extern "C" int cozo_gpu_sssp_goals(cozo_gpu_graph_t* g, const uint32_t* sources, uint32_t n_src, const uint32_t* goals,
+                                   uint32_t n_goals, int32_t keep_ties, float* out_cost, uint64_t* out_path_off,
+                                   uint32_t* out_paths, uint64_t paths_cap, uint64_t* out_tie_off,
+                                   uint32_t* out_tie_edges, uint64_t ties_cap, double* out_kernel_ms,
+                                   const volatile int* poison) {
+  const uint64_t pairs = (uint64_t)n_src * n_goals;
+  uint64_t* off_out = keep_ties ? out_tie_off : out_path_off;
+  uint32_t* rows_out = keep_ties ? out_tie_edges : out_paths;
+  const uint64_t cap = keep_ties ? ties_cap : paths_cap;
+  if (!g || (n_src && !sources) || (n_goals && !goals) || (pairs && !out_cost) || !off_out || (cap && !rows_out))
+    return set_error(COZO_GPU_EINVAL, "null argument");
+  int rc = ensure_init();
+  if (rc) return rc;
+  if (out_kernel_ms) *out_kernel_ms = 0;
+  rc = sssp_goals_check(g, sources, n_src, goals, n_goals);
+  if (rc) return rc;
+  // offsets per pair (paths) or per source (tied edges); a source with no goals has none of either
+  const uint64_t n_off = keep_ties ? (uint64_t)n_src + 1 : pairs + 1;
+  std::fill(off_out, off_out + n_off, 0);
+  if (pairs == 0) return 0;
+  CallStream cs;
+  rc = cs.init();
+  if (rc) return rc;
+  const uint64_t per_row = keep_ties ? 2 : 1;
+  rc = sssp_goals_run(g, cs, sources, n_src, goals, n_goals, keep_ties != 0, out_cost, off_out, cap, poison,
+                      [&](const uint32_t* drows, uint64_t base, uint64_t total) -> int {
+                        COZO_CUDA(cudaMemcpyAsync(rows_out + base * per_row, drows, total * per_row * 4,
+                                                  cudaMemcpyDeviceToHost, cs.s));
+                        return 0;
+                      });
   const double ms = cs.stop();
   if (out_kernel_ms) *out_kernel_ms = ms;
   return rc;
+}
+
+int cozo::closeness_run(cozo_gpu_graph_t* g, CallStream& cs, uint32_t lo, uint32_t hi, float* dout,
+                        const volatile int* poison) {
+  const uint32_t n = g->n;
+  std::vector<uint32_t> sources(hi - lo);
+  for (uint32_t i = lo; i < hi; ++i) sources[i - lo] = i;
+  return sssp_chunks(g, cs, sources.data(), hi - lo, 0, poison,
+                     [&](uint32_t s0, uint32_t c, unsigned long long* state, uint32_t*) -> int {
+                       closeness_kernel<<<c, 256, 0, cs.s>>>(state, n, c, s0, dout);
+                       return 0;
+                     });
 }
 
 extern "C" int cozo_gpu_closeness(cozo_gpu_graph_t* g, float* out, double* out_kernel_ms,
@@ -486,24 +515,44 @@ extern "C" int cozo_gpu_closeness(cozo_gpu_graph_t* g, float* out, double* out_k
   if (out_kernel_ms) *out_kernel_ms = 0;
   const uint32_t n = g->n;
   if (n == 0) return 0;  // all_pairs_shortest_path.rs:111-113
-  std::vector<uint32_t> sources(n);
-  for (uint32_t i = 0; i < n; ++i) sources[i] = i;
   CallStream cs;
   rc = cs.init();
   if (rc) return rc;
   DevBuf dout;
   COZO_CUDA(cudaMalloc(&dout.p, (size_t)n * 4));
-  rc = sssp_chunks(g, cs, sources.data(), n, 0, poison,
-                   [&](uint32_t s0, uint32_t c, unsigned long long* state, uint32_t*) -> int {
-                     closeness_kernel<<<c, 256, 0, cs.s>>>(state, n, c, s0, dout.as<float>());
-                     return 0;
-                   });
+  rc = closeness_run(g, cs, 0, n, dout.as<float>(), poison);
   const double ms = cs.stop();
   if (out_kernel_ms) *out_kernel_ms = ms;
   if (rc) return rc;
   COZO_CUDA(cudaMemcpyAsync(out, dout.p, (size_t)n * 4, cudaMemcpyDeviceToHost, cs.s));
   COZO_CUDA(cudaStreamSynchronize(cs.s));
   return 0;
+}
+
+int cozo::betweenness_run(cozo_gpu_graph_t* g, CallStream& cs, uint32_t lo, uint32_t hi, double* dbc, int* dcyc,
+                          const volatile int* poison) {
+  const uint32_t n = g->n;
+  std::vector<uint32_t> sources(hi - lo);
+  for (uint32_t i = lo; i < hi; ++i) sources[i - lo] = i;
+  DevBuf sig, del;
+  size_t sig_cap = 0;
+  return sssp_chunks(g, cs, sources.data(), hi - lo, (size_t)n * 32, poison,
+                     [&](uint32_t, uint32_t c, unsigned long long* state, uint32_t* dsrc) -> int {
+                       size_t need = (size_t)c * 2 * n * 8;
+                       if (sig_cap < need) {
+                         COZO_CUDA(cudaStreamSynchronize(cs.s));
+                         if (sig.p) cudaFree(sig.p);
+                         if (del.p) cudaFree(del.p);
+                         sig.p = del.p = nullptr;
+                         COZO_CUDA(cudaMalloc(&sig.p, need));
+                         COZO_CUDA(cudaMalloc(&del.p, need));
+                         sig_cap = need;
+                       }
+                       betweenness_kernel<<<c, 256, 0, cs.s>>>(g->out_ptr, g->out_idx, g->out_w, n, dsrc, c, state,
+                                                              sig.as<double>(), del.as<double>(), dcyc);
+                       betweenness_reduce_kernel<<<(n + 255) / 256, 256, 0, cs.s>>>(del.as<double>(), n, c, dbc);
+                       return 0;
+                     });
 }
 
 extern "C" int cozo_gpu_betweenness(cozo_gpu_graph_t* g, float* out, double* out_kernel_ms,
@@ -514,35 +563,16 @@ extern "C" int cozo_gpu_betweenness(cozo_gpu_graph_t* g, float* out, double* out
   if (out_kernel_ms) *out_kernel_ms = 0;
   const uint32_t n = g->n;
   if (n == 0) return 0;  // all_pairs_shortest_path.rs:43-46
-  std::vector<uint32_t> sources(n);
-  for (uint32_t i = 0; i < n; ++i) sources[i] = i;
   CallStream cs;
   rc = cs.init();
   if (rc) return rc;
-  DevBuf bc, bcf, sig, del, cyc;
+  DevBuf bc, bcf, cyc;
   COZO_CUDA(cudaMalloc(&bc.p, (size_t)n * 8));
   COZO_CUDA(cudaMemsetAsync(bc.p, 0, (size_t)n * 8, cs.s));
   COZO_CUDA(cudaMalloc(&bcf.p, (size_t)n * 4));
   COZO_CUDA(cudaMalloc(&cyc.p, 4));
   COZO_CUDA(cudaMemsetAsync(cyc.p, 0, 4, cs.s));
-  size_t sig_cap = 0;
-  rc = sssp_chunks(g, cs, sources.data(), n, (size_t)n * 32, poison,
-                   [&](uint32_t, uint32_t c, unsigned long long* state, uint32_t* dsrc) -> int {
-                     size_t need = (size_t)c * 2 * n * 8;
-                     if (sig_cap < need) {
-                       COZO_CUDA(cudaStreamSynchronize(cs.s));
-                       if (sig.p) cudaFree(sig.p);
-                       if (del.p) cudaFree(del.p);
-                       sig.p = del.p = nullptr;
-                       COZO_CUDA(cudaMalloc(&sig.p, need));
-                       COZO_CUDA(cudaMalloc(&del.p, need));
-                       sig_cap = need;
-                     }
-                     betweenness_kernel<<<c, 256, 0, cs.s>>>(g->out_ptr, g->out_idx, g->out_w, n, dsrc, c, state,
-                                                            sig.as<double>(), del.as<double>(), cyc.as<int>());
-                     betweenness_reduce_kernel<<<(n + 255) / 256, 256, 0, cs.s>>>(del.as<double>(), n, c, bc.as<double>());
-                     return 0;
-                   });
+  rc = betweenness_run(g, cs, 0, n, bc.as<double>(), cyc.as<int>(), poison);
   int hcyc = 0;
   if (!rc) {
     f64_to_f32_kernel<<<(n + 255) / 256, 256, 0, cs.s>>>(bc.as<double>(), n, bcf.as<float>());

@@ -1,5 +1,6 @@
 // graph_host.hpp — host-side state of a staged graph (opaque cozo_gpu_graph_t).
 #pragma once
+#include <functional>
 #include <mutex>
 
 #include "common.cuh"
@@ -72,4 +73,28 @@ namespace cozo {
 // CSR on `g`, in `st`.  Validates ids and weights; returns 0 or a COZO_GPU_E* code with the message set.  The caller
 // frees `g` on failure.
 int graph_build_csr(cozo_gpu_graph_t* g, const uint32_t* dsrc, const uint32_t* ddst, const float* dw, cudaStream_t st);
+
+// The source-parallel bodies of the all-source and many-source calls, over any slice of their sources, so that the
+// single-GPU entry points (the whole range) and the sharded ones (graph replicated, sources split over the ranks,
+// sharded.cu) run the same code.  All run on cs.s, poll `poison` between source chunks and return 0 or a
+// COZO_GPU_E* code with the message set.
+// closeness of the sources [lo, hi) into dout[0 .. hi - lo) (device memory)
+int closeness_run(cozo_gpu_graph_t* g, CallStream& cs, uint32_t lo, uint32_t hi, float* dout,
+                  const volatile int* poison);
+// the dependencies of the sources [lo, hi) added to dbc[n] (device f64) one source after the other, in source order;
+// *dcyc (device) is set when a zero-weight cycle of tied paths is met
+int betweenness_run(cozo_gpu_graph_t* g, CallStream& cs, uint32_t lo, uint32_t hi, double* dbc, int* dcyc,
+                    const volatile int* poison);
+// cozo_gpu_sssp_goals' argument checks on sources and goals
+int sssp_goals_check(cozo_gpu_graph_t* g, const uint32_t* sources, uint32_t n_src, const uint32_t* goals,
+                     uint32_t n_goals);
+// rows of one source chunk, on the device: rows [base, base + total) of the call's row list, each one path node (one
+// u32) or one (v, p) tie edge (two u32), ordered on cs.s
+using GoalRowSink = std::function<int(const uint32_t* drows, uint64_t base, uint64_t total)>;
+// cozo_gpu_sssp_goals for the given sources (host memory, checked): costs into out_cost (host), offsets into off_out
+// (host, n_src * n_goals + 1 or, with keep_ties, n_src + 1 entries, starting at 0).  The rows of every chunk go to
+// `sink` while the rows so far fit `cap`; after the first chunk that does not fit, only costs and offsets follow.
+int sssp_goals_run(cozo_gpu_graph_t* g, CallStream& cs, const uint32_t* sources, uint32_t n_src, const uint32_t* goals,
+                   uint32_t n_goals, bool keep_ties, float* out_cost, uint64_t* off_out, uint64_t cap,
+                   const volatile int* poison, const GoalRowSink& sink);
 }  // namespace cozo

@@ -1,4 +1,6 @@
-// sharded.cu — the row-sharded corpus behind the C ABI (SURVEY.md §8b "Multi-GPU", §8e):
+// sharded.cu — the row-sharded corpus behind the C ABI (SURVEY.md §8b "Multi-GPU", §8e), and the source-sharded
+// graph calls at the end of this file (replicated graph, sources split over the ranks, one exchange at the end).
+// The HNSW corpus:
 // one process per GPU, every rank holds one shard (its own vectors + its own HNSW graph).
 //   cozo_gpu_hnsw_search_sharded = query broadcast -> per-shard hnsw_knn -> exchange of the
 //   per-shard top-k lists -> k-way merge to global ids, all inside libcozo_gpu.so.
@@ -22,6 +24,7 @@
 #include <type_traits>
 #include <vector>
 
+#include "graph_host.hpp"
 #include "hnsw_host.hpp"
 
 namespace cozo {
@@ -116,7 +119,13 @@ struct cozo_gpu_shards {
   size_t out_rows = 0, out_k = 0;
   uint32_t* d_mask = nullptr;  // row filter verdicts of the host-pointer call, uploaded once per call
   size_t mask_words = 0;
-  std::mutex mu;  // one sharded search at a time per communicator (collectives must not interleave)
+  // the replicated graph of the sharded graph calls (cozo_gpu_graph_attach_sharded); not owned
+  cozo_gpu_graph* graph = nullptr;
+  uint64_t graph_sum = 0;  // its checksum, agreed at attach
+  // the status records of the sharded graph calls: [world + 1] records of 128 bytes, allocated with the group so
+  // that no call has to allocate before its status all-gather; the last one is scratch
+  uint8_t* d_status = nullptr;
+  std::mutex mu;  // one sharded call at a time per communicator (collectives must not interleave)
 };
 
 namespace cozo {
@@ -394,7 +403,8 @@ extern "C" int cozo_gpu_shards_init(cozo_gpu_shards_t** out, const uint8_t* id, 
   };
   if (cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking) != cudaSuccess ||
       cudaMalloc(&s->d_timeout, 4) != cudaSuccess || cudaMemset(s->d_timeout, 0, 4) != cudaSuccess ||
-      cudaMalloc(&s->d_offsets, (size_t)world * 8) != cudaSuccess)
+      cudaMalloc(&s->d_offsets, (size_t)world * 8) != cudaSuccess ||
+      cudaMalloc(&s->d_status, 128 * ((size_t)world + 1)) != cudaSuccess)
     return fail(set_error(COZO_GPU_ECUDA, "shard group creation failed: %s", cudaGetErrorString(cudaGetLastError())));
   ncclUniqueId u;
   memcpy(&u, id, sizeof(u));
@@ -409,7 +419,8 @@ extern "C" void cozo_gpu_shards_free(cozo_gpu_shards_t* s) {
   if (s->stream) cudaStreamSynchronize(s->stream);
   close_peers(s);
   void* ptrs[] = {s->block,    s->local_ids[0], s->local_ids[1], s->local_dist[0], s->local_dist[1], s->d_offsets,
-                  s->d_timeout, s->d_q,         s->d_out_ids,    s->d_out_dist,    s->d_qstats,      s->d_mask};
+                  s->d_timeout, s->d_q,         s->d_out_ids,    s->d_out_dist,    s->d_qstats,      s->d_mask,
+                  s->d_status};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   if (s->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(s->comm);
@@ -648,4 +659,411 @@ extern "C" int cozo_gpu_hnsw_search_sharded_f64(cozo_gpu_shards_t* s, const doub
                                                 CozoGpuSearchStats* stats) {
   return sharded_host_entry<double>(s, queries, B, k, ef, radius, root, false, row_mask, out_ids, out_dist, out_count,
                                     stats);
+}
+
+// ---- source-sharded graph calls: the graph is replicated, the sources are split ---------------------------------
+// SURVEY.md §8e "replicate graph, partition sources; no exchange until the end".  Every rank stages the same graph and
+// attaches it; the sources of a call are split into `world` contiguous slices in source order, rank r searches slice r
+// with the single-GPU code (graph.cu: closeness_run, betweenness_run, sssp_goals_run) and the slices are exchanged
+// once at the end, so every rank returns the whole answer.
+// Every call, attach included, starts its collectives with one all-gather of a fixed-size status record: this rank's
+// outcome (argument checks, poison, out of memory, ...) and the call's signature (which call, which graph, and every
+// argument that sizes a later collective).  All ranks then take the same branch: when the signatures differ — the
+// ranks made different calls, e.g. two rules run concurrently in different orders — every rank returns EINVAL, and
+// when a rank failed every rank returns that rank's code, so no rank meets a peer in a collective of another size or
+// waits for one that never comes.  Buffers a call needs are allocated before its status all-gather; the one whose size
+// is known only after it (the rows of sssp_goals) reports its allocation in the next all-gather.
+namespace cozo {
+
+__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {  // the splitmix64 finaliser
+  x ^= x >> 30;
+  x *= 0xBF58476D1CE4E5B9ull;
+  x ^= x >> 27;
+  x *= 0x94D049BB133111EBull;
+  return x ^ (x >> 31);
+}
+
+// order-free checksum of one array of 32-bit words: the sum of mix64(position, salt, word) (wrapping), so the same
+// bits give the same value whatever the launch geometry or the order of the atomics
+__global__ void graph_checksum_kernel(const uint32_t* a, uint64_t count, uint64_t salt, unsigned long long* out) {
+  unsigned long long acc = 0;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (uint64_t)gridDim.x * blockDim.x)
+    acc += mix64(mix64(i * 4 + salt) ^ a[i]);
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) atomicAdd(out, acc);
+}
+
+// betweenness: the ranks' f64 partial sums [world][n] added in rank order, rounded to f32 once
+__global__ void bc_rank_sum_kernel(const double* parts, uint32_t n, uint32_t world, float* out) {
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n) return;
+  double acc = parts[v];
+  for (uint32_t r = 1; r < world; ++r) acc += parts[(size_t)r * n + v];
+  out[v] = (float)acc;
+}
+
+// slice r of `total` sources: [total * r / world, total * (r + 1) / world); no slice is longer than ceil(total / world)
+static void source_slice(uint32_t total, int world, int r, uint32_t& lo, uint32_t& hi) {
+  lo = (uint32_t)((uint64_t)total * (uint64_t)r / (uint64_t)world);
+  hi = (uint32_t)((uint64_t)total * (uint64_t)(r + 1) / (uint64_t)world);
+}
+
+// all-gather of `count` elements per rank on the group's stream; in place when send == recv + rank * count
+static int group_all_gather(cozo_gpu_shards* s, const void* send, void* recv, size_t count, ncclDataType_t t,
+                            size_t elem) {
+  if (s->world > 1)
+    COZO_NCCL(g_nccl.AllGather(send, recv, count, t, s->comm, s->stream));
+  else if (send != recv)
+    COZO_CUDA(cudaMemcpyAsync(recv, send, count * elem, cudaMemcpyDeviceToDevice, s->stream));
+  return 0;
+}
+
+enum GraphCall : uint64_t { CALL_ATTACH = 1, CALL_CLOSENESS, CALL_BETWEENNESS, CALL_SSSP_GOALS };
+constexpr int kSigWords = 12;
+static const char* const kCallNames[] = {"no call", "attach", "closeness", "betweenness", "sssp_goals"};
+static const char* const kSigNames[kSigWords] = {"the call",        "n",           "m",         "weighted",
+                                                 "graph checksum",  "n_src",       "n_goals",   "keep_ties",
+                                                 "row capacity",    "the sources and goals", "", ""};
+
+// one rank's status record: its outcome, then the call's signature
+struct CallRecord {
+  int64_t rc = 0, cyclic = 0, rows = 0, pad = 0;  // return code, zero-weight-cycle flag, rows of its slice
+  // call kind, n, m, weighted, graph checksum, n_src, n_goals, keep_ties, cap, hash of sources and goals, 0, 0
+  uint64_t sig[kSigWords] = {};
+};
+static_assert(sizeof(CallRecord) == 128, "one 128-byte record per rank (cozo_gpu_shards::d_status)");
+
+// the signature of a call on the attached graph (all zero but the kind when none is attached)
+static CallRecord graph_record(const cozo_gpu_shards* s, uint64_t kind) {
+  CallRecord r;
+  r.sig[0] = kind;
+  if (s->graph) {
+    r.sig[1] = s->graph->n;
+    r.sig[2] = s->graph->m;
+    r.sig[3] = s->graph->weighted ? 1 : 0;
+    r.sig[4] = s->graph_sum;
+  }
+  return r;
+}
+
+static uint64_t fnv1a(uint64_t h, const void* p, size_t bytes) {
+  const uint8_t* b = static_cast<const uint8_t*>(p);
+  for (size_t i = 0; i < bytes; ++i) h = (h ^ b[i]) * 0x100000001B3ull;
+  return h;
+}
+
+// The one status all-gather of a sharded graph call.  Returns 0 when every rank succeeded with the same signature;
+// otherwise, on every rank, EINVAL when the signatures differ, else the code of the first failing rank in rank order.
+static int exchange_status(cozo_gpu_shards* s, const CallRecord& mine, std::vector<CallRecord>& all) {
+  CallRecord* d = reinterpret_cast<CallRecord*>(s->d_status);
+  COZO_CUDA(cudaMemcpyAsync(d + s->rank, &mine, sizeof(CallRecord), cudaMemcpyHostToDevice, s->stream));
+  int rc = group_all_gather(s, d + s->rank, d, sizeof(CallRecord), ncclUint8, 1);
+  if (rc) return rc;
+  all.resize(s->world);
+  COZO_CUDA(cudaMemcpyAsync(all.data(), d, sizeof(CallRecord) * (size_t)s->world, cudaMemcpyDeviceToHost, s->stream));
+  COZO_CUDA(cudaStreamSynchronize(s->stream));
+  for (int r = 1; r < s->world; ++r)
+    for (int k = 0; k < kSigWords; ++k)
+      if (all[r].sig[k] != all[0].sig[k])
+        return set_error(COZO_GPU_EINVAL,
+                         "the ranks of the shard group made different calls (rank 0: %s, rank %d: %s; they differ in %s): "
+                         "every rank must make the same call with the same arguments on the same graph",
+                         kCallNames[std::min<uint64_t>(all[0].sig[0], 4)], r,
+                         kCallNames[std::min<uint64_t>(all[r].sig[0], 4)], kSigNames[k]);
+  for (int r = 0; r < s->world; ++r) {
+    if (!all[r].rc) continue;
+    if (r != s->rank)  // the failing rank keeps its own message
+      set_error((int)all[r].rc, "rank %d of the shard group failed (code %d); the sharded call stops on every rank", r,
+                (int)all[r].rc);
+    return (int)all[r].rc;
+  }
+  return 0;
+}
+
+static int check_graph_group(const cozo_gpu_shards* s) {
+  if (!s->graph) return set_error(COZO_GPU_EINVAL, "no graph attached to the shard group (cozo_gpu_graph_attach_sharded)");
+  return 0;
+}
+
+// a rank with an empty slice runs no source chunk; it still answers its poison flag
+static int poll_poison(const volatile int* poison) {
+  return poisoned(poison) ? set_error(COZO_GPU_EKILLED, "Running query is killed before completion") : 0;
+}
+
+}  // namespace cozo
+
+extern "C" int cozo_gpu_graph_attach_sharded(cozo_gpu_shards_t* s, cozo_gpu_graph_t* g) {
+  if (!s) return set_error(COZO_GPU_EINVAL, "null argument");
+  int rc = ensure_init();
+  if (rc) return rc;
+  std::lock_guard<std::mutex> lk(s->mu);
+  s->graph = nullptr;
+  s->graph_sum = 0;
+  CallRecord rec;
+  rec.sig[0] = CALL_ATTACH;
+  auto local = [&]() -> int {
+    if (!g) return set_error(COZO_GPU_EINVAL, "null graph handle");
+    cudaStream_t st = s->stream;
+    // checksum of out_ptr, out_idx and the bits of out_w, accumulated in the scratch record
+    auto* sum = reinterpret_cast<unsigned long long*>(s->d_status + 128 * (size_t)s->world);
+    COZO_CUDA(cudaMemsetAsync(sum, 0, 8, st));
+    const struct {
+      const uint32_t* a;
+      uint64_t count;
+    } parts[3] = {{g->out_ptr, (uint64_t)g->n + 1},
+                  {g->out_idx, g->m},
+                  {reinterpret_cast<const uint32_t*>(g->out_w), g->weighted ? g->m : 0}};
+    for (int i = 0; i < 3; ++i) {
+      if (!parts[i].a || !parts[i].count) continue;
+      const uint32_t blocks = (uint32_t)std::min<uint64_t>((parts[i].count + 255) / 256, 1024);
+      graph_checksum_kernel<<<blocks, 256, 0, st>>>(parts[i].a, parts[i].count, (uint64_t)i << 62, sum);
+    }
+    COZO_CUDA(cudaGetLastError());
+    unsigned long long h = 0;
+    COZO_CUDA(cudaMemcpyAsync(&h, sum, 8, cudaMemcpyDeviceToHost, st));
+    COZO_CUDA(cudaStreamSynchronize(st));
+    rec.sig[1] = g->n;
+    rec.sig[2] = g->m;
+    rec.sig[3] = g->weighted ? 1 : 0;
+    rec.sig[4] = h;
+    return 0;
+  };
+  rec.rc = local();
+  std::vector<CallRecord> all;
+  rc = exchange_status(s, rec, all);  // graphs that differ: EINVAL on every rank, and the group keeps no graph
+  if (rc) return rc;
+  s->graph = g;
+  s->graph_sum = rec.sig[4];
+  return 0;
+}
+
+extern "C" int cozo_gpu_closeness_sharded(cozo_gpu_shards_t* s, float* out, double* out_kernel_ms,
+                                          const volatile int* poison) {
+  if (!s) return set_error(COZO_GPU_EINVAL, "null argument");
+  int rc = ensure_init();
+  if (rc) return rc;
+  if (out_kernel_ms) *out_kernel_ms = 0;
+  std::lock_guard<std::mutex> lk(s->mu);
+  CallRecord rec = graph_record(s, CALL_CLOSENESS);
+  cozo_gpu_graph* g = s->graph;
+  const uint32_t n = g ? g->n : 0;
+  const uint32_t W = (uint32_t)s->world, cmax = (n + W - 1) / W;
+  uint32_t lo, hi;
+  source_slice(n, s->world, s->rank, lo, hi);
+  CallStream cs;
+  DevBuf dall;  // [world][cmax]: slice r at row r
+  auto local = [&]() -> int {
+    if (!out) return set_error(COZO_GPU_EINVAL, "null argument");
+    int e = check_graph_group(s);
+    if (e || n == 0) return e;  // n == 0: all_pairs_shortest_path.rs:111-113
+    COZO_CUDA(cudaMalloc(&dall.p, (size_t)W * cmax * 4));
+    e = cs.init();
+    if (e) return e;
+    if (hi == lo) return poll_poison(poison);
+    return closeness_run(g, cs, lo, hi, dall.as<float>() + (size_t)s->rank * cmax, poison);
+  };
+  rec.rc = local();
+  const double ms = cs.e1 ? cs.stop() : 0.0;
+  if (out_kernel_ms) *out_kernel_ms = ms;
+  std::vector<CallRecord> all;
+  rc = exchange_status(s, rec, all);
+  if (rc || n == 0) return rc;
+  rc = group_all_gather(s, dall.as<float>() + (size_t)s->rank * cmax, dall.p, cmax, ncclFloat32, 4);
+  if (rc) return rc;
+  std::vector<float> h((size_t)W * cmax);
+  COZO_CUDA(cudaMemcpyAsync(h.data(), dall.p, h.size() * 4, cudaMemcpyDeviceToHost, s->stream));
+  COZO_CUDA(cudaStreamSynchronize(s->stream));
+  for (int r = 0; r < s->world; ++r) {
+    uint32_t a, b;
+    source_slice(n, s->world, r, a, b);
+    std::copy(h.begin() + (size_t)r * cmax, h.begin() + (size_t)r * cmax + (b - a), out + a);
+  }
+  return 0;
+}
+
+extern "C" int cozo_gpu_betweenness_sharded(cozo_gpu_shards_t* s, float* out, double* out_kernel_ms,
+                                            const volatile int* poison) {
+  if (!s) return set_error(COZO_GPU_EINVAL, "null argument");
+  int rc = ensure_init();
+  if (rc) return rc;
+  if (out_kernel_ms) *out_kernel_ms = 0;
+  std::lock_guard<std::mutex> lk(s->mu);
+  CallRecord rec = graph_record(s, CALL_BETWEENNESS);
+  cozo_gpu_graph* g = s->graph;
+  const uint32_t n = g ? g->n : 0;
+  uint32_t lo, hi;
+  source_slice(n, s->world, s->rank, lo, hi);
+  CallStream cs;
+  DevBuf dall, dcyc, dout;  // dall: [world][n] f64 partial sums, this rank's at row `rank`
+  double* mine = nullptr;
+  int hcyc = 0;
+  auto local = [&]() -> int {
+    if (!out) return set_error(COZO_GPU_EINVAL, "null argument");
+    int e = check_graph_group(s);
+    if (e || n == 0) return e;  // n == 0: all_pairs_shortest_path.rs:43-46
+    COZO_CUDA(cudaMalloc(&dall.p, (size_t)s->world * n * 8));
+    COZO_CUDA(cudaMalloc(&dcyc.p, 4));
+    COZO_CUDA(cudaMalloc(&dout.p, (size_t)n * 4));
+    e = cs.init();
+    if (e) return e;
+    mine = dall.as<double>() + (size_t)s->rank * n;
+    COZO_CUDA(cudaMemsetAsync(mine, 0, (size_t)n * 8, cs.s));
+    COZO_CUDA(cudaMemsetAsync(dcyc.p, 0, 4, cs.s));
+    e = hi > lo ? betweenness_run(g, cs, lo, hi, mine, dcyc.as<int>(), poison) : poll_poison(poison);
+    if (e) return e;
+    COZO_CUDA(cudaMemcpyAsync(&hcyc, dcyc.p, 4, cudaMemcpyDeviceToHost, cs.s));
+    COZO_CUDA(cudaStreamSynchronize(cs.s));
+    return 0;
+  };
+  rec.rc = local();
+  rec.cyclic = hcyc;
+  const double ms = cs.e1 ? cs.stop() : 0.0;
+  if (out_kernel_ms) *out_kernel_ms = ms;
+  std::vector<CallRecord> all;
+  rc = exchange_status(s, rec, all);
+  if (rc || n == 0) return rc;
+  for (const CallRecord& x : all)
+    if (x.cyclic)
+      return set_error(COZO_GPU_EUNSUP, "betweenness: a zero-weight cycle makes the set of tied shortest paths unbounded "
+                                        "(the reference does not terminate on this input)");
+  rc = group_all_gather(s, mine, dall.p, n, ncclFloat64, 8);
+  if (rc) return rc;
+  bc_rank_sum_kernel<<<(n + 255) / 256, 256, 0, s->stream>>>(dall.as<double>(), n, (uint32_t)s->world, dout.as<float>());
+  COZO_CUDA(cudaGetLastError());
+  COZO_CUDA(cudaMemcpyAsync(out, dout.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s->stream));
+  COZO_CUDA(cudaStreamSynchronize(s->stream));
+  return 0;
+}
+
+extern "C" int cozo_gpu_sssp_goals_sharded(cozo_gpu_shards_t* s, const uint32_t* sources, uint32_t n_src,
+                                           const uint32_t* goals, uint32_t n_goals, int32_t keep_ties, float* out_cost,
+                                           uint64_t* out_path_off, uint32_t* out_paths, uint64_t paths_cap,
+                                           uint64_t* out_tie_off, uint32_t* out_tie_edges, uint64_t ties_cap,
+                                           double* out_kernel_ms, const volatile int* poison) {
+  const uint64_t pairs = (uint64_t)n_src * n_goals;
+  uint64_t* off_out = keep_ties ? out_tie_off : out_path_off;
+  uint32_t* rows_out = keep_ties ? out_tie_edges : out_paths;
+  const uint64_t cap = keep_ties ? ties_cap : paths_cap;
+  if (!s) return set_error(COZO_GPU_EINVAL, "null argument");
+  int rc = ensure_init();
+  if (rc) return rc;
+  if (out_kernel_ms) *out_kernel_ms = 0;
+  std::lock_guard<std::mutex> lk(s->mu);
+  cozo_gpu_graph* g = s->graph;
+  CallRecord rec = graph_record(s, CALL_SSSP_GOALS);
+  rec.sig[5] = n_src;
+  rec.sig[6] = n_goals;
+  rec.sig[7] = keep_ties ? 1 : 0;
+  rec.sig[8] = cap;
+  rec.sig[9] = 0xCBF29CE484222325ull;
+  if (sources) rec.sig[9] = fnv1a(rec.sig[9], sources, (size_t)n_src * 4);
+  if (goals) rec.sig[9] = fnv1a(rec.sig[9], goals, (size_t)n_goals * 4);
+  const uint32_t W = (uint32_t)s->world, cmax = (n_src + W - 1) / W;
+  uint32_t lo, hi;
+  source_slice(n_src, s->world, s->rank, lo, hi);
+  const uint64_t per_row = keep_ties ? 2 : 1;          // u32 per row
+  const uint64_t per_src = keep_ties ? 1 : n_goals;    // offsets per source
+  // one slot per rank: costs [cmax * n_goals]; offsets [cmax * per_src + 1], then one word = "my row buffer is ready"
+  const uint64_t slot_off = (uint64_t)cmax * per_src + 2, slot_cost = (uint64_t)cmax * n_goals;
+  std::vector<float> lcost(slot_cost);
+  std::vector<uint64_t> loff(slot_off, 0);
+  DevBuf dlocal, dcost, doff;  // this rank's rows; every slot's costs and offsets
+  uint64_t local_cap = 0;      // rows dlocal holds
+  CallStream cs;
+  auto local = [&]() -> int {
+    if ((n_src && !sources) || (n_goals && !goals) || (pairs && !out_cost) || !off_out || (cap && !rows_out))
+      return set_error(COZO_GPU_EINVAL, "null argument");
+    int e = check_graph_group(s);
+    if (!e) e = sssp_goals_check(g, sources, n_src, goals, n_goals);
+    if (e || pairs == 0) return e;
+    COZO_CUDA(cudaMalloc(&dcost.p, W * slot_cost * 4));
+    COZO_CUDA(cudaMalloc(&doff.p, W * slot_off * 8));
+    e = cs.init();
+    if (e) return e;
+    if (hi == lo) return poll_poison(poison);
+    return sssp_goals_run(
+        g, cs, sources + lo, hi - lo, goals, n_goals, keep_ties != 0, lcost.data(), loff.data(), cap, poison,
+        [&](const uint32_t* drows, uint64_t base, uint64_t total) -> int {
+          if (local_cap < base + total) {
+            DevBuf grown;
+            const uint64_t want = std::max(base + total, 2 * local_cap);
+            COZO_CUDA(cudaMalloc(&grown.p, want * per_row * 4));
+            if (base) COZO_CUDA(cudaMemcpyAsync(grown.p, dlocal.p, base * per_row * 4, cudaMemcpyDeviceToDevice, cs.s));
+            COZO_CUDA(cudaStreamSynchronize(cs.s));
+            std::swap(grown.p, dlocal.p);
+            local_cap = want;
+          }
+          COZO_CUDA(cudaMemcpyAsync(dlocal.as<uint32_t>() + base * per_row, drows, total * per_row * 4,
+                                    cudaMemcpyDeviceToDevice, cs.s));
+          return 0;
+        });
+  };
+  rec.rc = local();
+  rec.rows = (int64_t)(hi > lo ? loff[(uint64_t)(hi - lo) * per_src] : 0);
+  const double ms = cs.e1 ? cs.stop() : 0.0;
+  if (out_kernel_ms) *out_kernel_ms = ms;
+  std::vector<CallRecord> all;
+  rc = exchange_status(s, rec, all);
+  if (rc) return rc;
+  const uint64_t n_off = keep_ties ? (uint64_t)n_src + 1 : pairs + 1;
+  std::fill(off_out, off_out + n_off, 0);
+  if (pairs == 0) return 0;
+  std::vector<uint64_t> base(W + 1, 0);  // first row of every rank's slice; base[W] = the total
+  for (uint32_t r = 0; r < W; ++r) base[r + 1] = base[r] + (uint64_t)all[r].rows;
+  const uint64_t total = base[W];
+  const bool move_rows = total && total <= cap;  // as on one GPU: otherwise the caller retries with room for `total`
+  // the row buffer is sized by the total; whether every rank could allocate it travels with the offsets
+  DevBuf drows;
+  loff[slot_off - 1] = 1;
+  if (move_rows && cudaMalloc(&drows.p, total * per_row * 4) != cudaSuccess) {
+    cudaGetLastError();
+    loff[slot_off - 1] = 0;
+  }
+  // costs and offsets of every slice
+  float* my_cost = dcost.as<float>() + s->rank * slot_cost;
+  uint64_t* my_off = doff.as<uint64_t>() + s->rank * slot_off;
+  COZO_CUDA(cudaMemcpyAsync(my_cost, lcost.data(), slot_cost * 4, cudaMemcpyHostToDevice, s->stream));
+  COZO_CUDA(cudaMemcpyAsync(my_off, loff.data(), slot_off * 8, cudaMemcpyHostToDevice, s->stream));
+  if (W > 1) COZO_NCCL(g_nccl.GroupStart());
+  rc = group_all_gather(s, my_cost, dcost.p, slot_cost, ncclFloat32, 4);
+  if (!rc) rc = group_all_gather(s, my_off, doff.p, slot_off, ncclUint64, 8);
+  if (W > 1) COZO_NCCL(g_nccl.GroupEnd());
+  if (rc) return rc;
+  std::vector<float> hcost(W * slot_cost);
+  std::vector<uint64_t> hoff(W * slot_off);
+  COZO_CUDA(cudaMemcpyAsync(hcost.data(), dcost.p, hcost.size() * 4, cudaMemcpyDeviceToHost, s->stream));
+  COZO_CUDA(cudaMemcpyAsync(hoff.data(), doff.p, hoff.size() * 8, cudaMemcpyDeviceToHost, s->stream));
+  COZO_CUDA(cudaStreamSynchronize(s->stream));
+  for (uint32_t r = 0; r < W; ++r)
+    if (!hoff[r * slot_off + slot_off - 1])
+      return set_error(COZO_GPU_ENOMEM, "sssp_goals_sharded: rank %u could not allocate the %llu-row exchange buffer", r,
+                       (unsigned long long)total);
+  for (uint32_t r = 0; r < W; ++r) {
+    uint32_t a, b;
+    source_slice(n_src, s->world, (int)r, a, b);
+    std::copy(hcost.begin() + r * slot_cost, hcost.begin() + r * slot_cost + (uint64_t)(b - a) * n_goals,
+              out_cost + (uint64_t)a * n_goals);
+    const uint64_t* o = hoff.data() + r * slot_off;
+    for (uint64_t i = 0; b > a && i <= (uint64_t)(b - a) * per_src; ++i) off_out[a * per_src + i] = o[i] + base[r];
+  }
+  off_out[n_off - 1] = total;
+  if (!move_rows) return 0;
+  // the rows: one broadcast per rank of its slice's rows, into place
+  uint32_t* rows = drows.as<uint32_t>();
+  if (W > 1) {
+    COZO_NCCL(g_nccl.GroupStart());
+    for (uint32_t r = 0; r < W; ++r) {
+      const uint64_t cnt = base[r + 1] - base[r];
+      if (!cnt) continue;
+      uint32_t* dst = rows + base[r] * per_row;
+      COZO_NCCL(g_nccl.Broadcast((int)r == s->rank ? dlocal.p : dst, dst, cnt * per_row, ncclUint32, (int)r, s->comm,
+                                 s->stream));
+    }
+    COZO_NCCL(g_nccl.GroupEnd());
+  } else {
+    COZO_CUDA(cudaMemcpyAsync(rows, dlocal.p, total * per_row * 4, cudaMemcpyDeviceToDevice, s->stream));
+  }
+  COZO_CUDA(cudaMemcpyAsync(rows_out, rows, total * per_row * 4, cudaMemcpyDeviceToHost, s->stream));
+  COZO_CUDA(cudaStreamSynchronize(s->stream));
+  return 0;
 }

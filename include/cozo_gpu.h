@@ -399,6 +399,46 @@ int cozo_gpu_betweenness(cozo_gpu_graph_t* g, float* out, double* out_kernel_ms,
 int cozo_gpu_clustering(cozo_gpu_graph_t* g, double* out_cc, uint64_t* out_triangles, uint64_t* out_degree,
                         double* out_kernel_ms, const volatile int* poison);
 
+/* ---- source-sharded graph calls: the graph replicated on every rank, the sources split -----------------------
+ * SURVEY.md §8e "replicate graph, partition sources; no exchange until the end".  The shard group of
+ * cozo_gpu_shards_init, one process per GPU; every rank makes the same call with the same arguments.  The
+ * sources of a call are split into `world` contiguous slices in source order, slice r = [N*r/world,
+ * N*(r+1)/world) of the N sources (empty when world > N); rank r searches slice r with the single-GPU code and
+ * every rank returns the complete answer.  Each rank polls its own `poison` between source chunks (once when its
+ * slice is empty).  Every call, attach included, first all-gathers one status record per rank: its outcome and the
+ * call's signature (which call, the attached graph, n_src, n_goals, keep_ties, the row capacity and a hash of the
+ * sources and goals).  When the signatures differ — e.g. two calls reached the group in different orders on
+ * different ranks — every rank returns COZO_GPU_EINVAL; otherwise, when any rank failed (an argument check, no
+ * graph attached, poison, out of memory, ...), every rank returns the code of the first failing rank in rank
+ * order.  So no rank is left waiting, and the group stays usable.  Only a NULL `s` is refused on its rank alone.
+ * out_kernel_ms = device time of this rank's slice, before the exchange. */
+
+/* Collective.  Registers `g` — staged on every rank from the same edges with cozo_gpu_graph_stage or
+ * cozo_gpu_graph_stage_keys — on the group for the calls below.  Every rank all-gathers (n, m, weighted, a
+ * checksum computed on the device over the out-CSR and the bits of its weights); if any rank differs, every rank
+ * returns COZO_GPU_EINVAL and the group has no graph (on any rank whose attach fails).  The group does not own `g`: it must outlive its use
+ * through the group, and a re-staged graph is attached again. */
+int cozo_gpu_graph_attach_sharded(cozo_gpu_shards_t* s, cozo_gpu_graph_t* g);
+/* Collective.  cozo_gpu_closeness over the attached graph: the per-source f32 values of every slice are
+ * all-gathered, so `out` [n] equals cozo_gpu_closeness bit for bit at every world size. */
+int cozo_gpu_closeness_sharded(cozo_gpu_shards_t* s, float* out, double* out_kernel_ms, const volatile int* poison);
+/* Collective.  cozo_gpu_betweenness over the attached graph: each rank adds its slice's per-source dependencies in
+ * source order in f64, the world partial sums are all-gathered and every rank adds them in rank order and rounds
+ * to f32 once, so `out` [n] is the same on every rank and from run to run; at world 1 it equals
+ * cozo_gpu_betweenness bit for bit, above it only the association of the f64 sum differs.  COZO_GPU_EUNSUP on
+ * every rank when any rank met a zero-weight cycle of tied paths. */
+int cozo_gpu_betweenness_sharded(cozo_gpu_shards_t* s, float* out, double* out_kernel_ms, const volatile int* poison);
+/* Collective.  cozo_gpu_sssp_goals over the attached graph, with the same arguments, outputs and capacity rule:
+ * costs, offsets and rows equal the single-GPU call's (tie edges: the same multiset per source, in no particular
+ * order within a source).  Costs, offsets and every slice's row count are all-gathered, then each slice's rows
+ * are broadcast from its rank into place.  When the total exceeds paths_cap / ties_cap, costs and offsets are
+ * written and no row is. */
+int cozo_gpu_sssp_goals_sharded(cozo_gpu_shards_t* s, const uint32_t* sources, uint32_t n_src, const uint32_t* goals,
+                                uint32_t n_goals, int32_t keep_ties, float* out_cost, uint64_t* out_path_off,
+                                uint32_t* out_paths, uint64_t paths_cap, uint64_t* out_tie_off,
+                                uint32_t* out_tie_edges, uint64_t ties_cap, double* out_kernel_ms,
+                                const volatile int* poison);
+
 #ifdef __cplusplus
 }
 #endif

@@ -123,4 +123,8 @@ extern "C" {
     pub fn cozo_gpu_closeness(g: *mut CozoGpuGraph, out: *mut f32, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
     pub fn cozo_gpu_betweenness(g: *mut CozoGpuGraph, out: *mut f32, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
     pub fn cozo_gpu_clustering(g: *mut CozoGpuGraph, out_cc: *mut f64, out_triangles: *mut u64, out_degree: *mut u64, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
+    pub fn cozo_gpu_graph_attach_sharded(s: *mut CozoGpuShards, g: *mut CozoGpuGraph) -> c_int;
+    pub fn cozo_gpu_closeness_sharded(s: *mut CozoGpuShards, out: *mut f32, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
+    pub fn cozo_gpu_betweenness_sharded(s: *mut CozoGpuShards, out: *mut f32, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
+    pub fn cozo_gpu_sssp_goals_sharded(s: *mut CozoGpuShards, sources: *const u32, n_src: u32, goals: *const u32, n_goals: u32, keep_ties: i32, out_cost: *mut f32, out_path_off: *mut u64, out_paths: *mut u32, paths_cap: u64, out_tie_off: *mut u64, out_tie_edges: *mut u32, ties_cap: u64, out_kernel_ms: *mut f64, poison: *const c_int) -> c_int;
 }

@@ -50,6 +50,35 @@ pub(crate) fn ensure_device() -> Result<()> {
     }
 }
 
+/// Opt-in source sharding of ClosenessCentrality, BetweennessCentrality and ShortestPathDijkstra (with a termination
+/// relation) over a shard group: one process per GPU, every process runs the same query over the same relation, so
+/// each rank stages the same graph, searches its slice of the sources and returns the whole answer
+/// (cozo_gpu_graph_attach_sharded / cozo_gpu_*_sharded, INTEGRATION.md §5b).  The embedding process creates the group
+/// (cozo_gpu_shards_init) and registers it once; without it the rules run on one GPU.  The mutex keeps one rule's
+/// attach and call together: the group holds one attached graph at a time.
+///
+/// The rules of one stratum run concurrently (query/eval.rs:199-202), so two sharded rules may reach the group in a
+/// different order on different ranks.  The library detects that: every sharded call (attach included) all-gathers
+/// its signature first, and ranks whose calls differ all get COZO_GPU_EINVAL before any result collective.  The rule
+/// then answers on its own GPU, which gives the same rows; so does a rule whose graph differs between ranks.
+struct GraphShards(*mut CozoGpuShards);
+unsafe impl Send for GraphShards {}
+static GRAPH_SHARDS: std::sync::OnceLock<std::sync::Mutex<GraphShards>> = std::sync::OnceLock::new();
+
+pub fn set_graph_shards(grp: *mut CozoGpuShards) -> bool {
+    GRAPH_SHARDS.set(std::sync::Mutex::new(GraphShards(grp))).is_ok()
+}
+
+/// Return code of `call` on the registered group after attaching `g` to it; None when no group is registered or the
+/// group refused the attach or the call with COZO_GPU_EINVAL (the caller then runs the single-GPU entry point).
+fn with_graph_shards(g: &DevGraph, call: impl FnOnce(*mut CozoGpuShards) -> c_int) -> Option<c_int> {
+    let lock = GRAPH_SHARDS.get()?;
+    let grp = lock.lock().unwrap_or_else(|e| e.into_inner());
+    let rc = unsafe { cozo_gpu_graph_attach_sharded(grp.0, g.0) };
+    let rc = if rc == COZO_GPU_OK { call(grp.0) } else { rc };
+    if rc == COZO_GPU_EINVAL { None } else { Some(rc) }
+}
+
 /// Map a C-ABI return code to the error the reference raises on the same condition.
 fn check(rc: c_int) -> Result<()> {
     match rc {
@@ -369,12 +398,19 @@ impl FixedRule for ShortestPathDijkstraGpu {
             } else {
                 (off.as_mut_ptr(), rows.as_mut_ptr(), cap, ptr::null_mut(), ptr::null_mut(), 0)
             };
-            pm.guard(unsafe {
+            let rc = with_graph_shards(g, |grp| unsafe {
+                cozo_gpu_sssp_goals_sharded(
+                    grp, sources.as_ptr(), ns as u32, goals.as_ptr(), ng as u32, keep_ties as i32,
+                    cost.as_mut_ptr(), po, pp, pc, to, te, tc, &mut ms, pm.ptr(),
+                )
+            })
+            .unwrap_or_else(|| unsafe {
                 cozo_gpu_sssp_goals(
                     g.0, sources.as_ptr(), ns as u32, goals.as_ptr(), ng as u32, keep_ties as i32,
                     cost.as_mut_ptr(), po, pp, pc, to, te, tc, &mut ms, pm.ptr(),
                 )
-            })?;
+            });
+            pm.guard(rc)?;
             let total = *off.last().unwrap();
             if total <= cap {
                 break;
@@ -415,7 +451,7 @@ impl FixedRule for ShortestPathDijkstraGpu {
 // ClosenessCentrality / BetweennessCentrality (algos/all_pairs_shortest_path.rs:29-197)
 // ---------------------------------------------------------------------------------------------
 macro_rules! centrality_rule {
-    ($name:ident, $entry:ident) => {
+    ($name:ident, $entry:ident, $sharded:ident) => {
         pub(crate) struct $name;
         impl FixedRule for $name {
             fn run(&self, payload: FixedRulePayload<'_, '_>, out: &mut RegularTempStore, poison: Poison) -> Result<()> {
@@ -429,7 +465,9 @@ macro_rules! centrality_rule {
                 let pm = PoisonMirror::new(poison);
                 let mut res = vec![0f32; el.indices.len()];
                 let mut ms = 0f64;
-                pm.guard(unsafe { $entry(g.0, res.as_mut_ptr(), &mut ms, pm.ptr()) })?;
+                let rc = with_graph_shards(g, |grp| unsafe { $sharded(grp, res.as_mut_ptr(), &mut ms, pm.ptr()) })
+                    .unwrap_or_else(|| unsafe { $entry(g.0, res.as_mut_ptr(), &mut ms, pm.ptr()) });
+                pm.guard(rc)?;
                 for (i, s) in res.into_iter().enumerate() {
                     out.put(vec![el.indices[i].clone(), DataValue::from(s as f64)]);
                 }
@@ -441,8 +479,8 @@ macro_rules! centrality_rule {
         }
     };
 }
-centrality_rule!(ClosenessCentralityGpu, cozo_gpu_closeness);
-centrality_rule!(BetweennessCentralityGpu, cozo_gpu_betweenness);
+centrality_rule!(ClosenessCentralityGpu, cozo_gpu_closeness, cozo_gpu_closeness_sharded);
+centrality_rule!(BetweennessCentralityGpu, cozo_gpu_betweenness, cozo_gpu_betweenness_sharded);
 
 // ---------------------------------------------------------------------------------------------
 // ClusteringCoefficients (algos/triangles.rs:26-92): rows [node, coefficient, triangles, degree]
